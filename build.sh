@@ -2,7 +2,7 @@
 # Build / test driver -- counterpart of the reference's build.sh (build.sh:91-150 `unit_test`): native build, C++
 # stress test under sanitizers, unit tests, and the end-to-end matrix: examples standalone and with np in {1, 2},
 # checkpoint -> reload with a DIFFERENT worker count, one-batch edge cases. CPU / gloo only (the CI box has no GPU);
-# GPU tests: `./build.sh gpu` on a B200 box.
+# GPU tests: `./build.sh gpu` on an H100 machine.
 set -euo pipefail
 cd "$(dirname "$0")"
 PY=${PYTHON:-python}

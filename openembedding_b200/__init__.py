@@ -1,10 +1,10 @@
-"""openembedding_b200 -- a Blackwell-native sparse-embedding training/serving engine.
+"""openembedding_b200 -- a Hopper-native (H100, sm_90a) sparse-embedding training/serving engine.
 
 Same capabilities and Python surface as 4paradigm/OpenEmbedding (``Embedding``,
 ``Variable`` a.k.a. ``distributed_variable``, ``distributed_model``,
 ``distributed_optimizer``, server-model save/load, standalone export, ``flags``,
-``Master``/``Server``), rebuilt for one 8xB200 NVSwitch box on PyTorch: tables are
-row-sharded over the GPUs' HBM and pull / push+update are fused sm_100a kernels that
+``Master``/``Server``), rebuilt for one NVSwitch box of H100s on PyTorch: tables are
+row-sharded over the GPUs' HBM and pull / push+update are fused sm_90a kernels that
 talk to peer memory directly (see ``DESIGN.md``).
 
 Reference package root: openembedding/__init__.py:33-76.
@@ -21,7 +21,7 @@ class Flags:
         self.bind_ip = ""
         self.num_workers = 1
         self.wait_num_servers = -1  # -1: every worker hosts its shards in-process (the only GPU mode)
-        # B200 additions
+        # additions of this engine
         self.device = "auto"        # auto | cuda | cpu
         self.seed = 0               # Philox seed of the server-side initializers
 

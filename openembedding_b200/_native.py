@@ -4,7 +4,7 @@ Reference: the pybind11 module ``libexb`` (openembedding/entry/py_api.cc:225-...
 openembedding/entry/c_api.h; here the C ABI is called directly (ctypes releases the GIL on every call).
 
 ``core()`` -> ``libexb_core.so`` (CPU engine + checkpoint IO), ``cuda()`` ->
-``libexb_cuda.so`` (sm_100a kernels). Loading is lazy; a missing/stale library is
+``libexb_cuda.so`` (sm_90a kernels). Loading is lazy; a missing/stale library is
 rebuilt if a compiler is present, otherwise an ImportError explains what is missing --
 on a GPU box the CUDA ops never silently fall back to eager PyTorch.
 """

@@ -1,6 +1,6 @@
 """Sparse-table backends behind ``Context``.
 
-* ``CudaBackend`` -- the product: HBM shards + fused sm_100a kernels + NVLink peer memory
+* ``CudaBackend`` -- the product: HBM shards + fused sm_90a kernels + NVLink peer memory
   (``ops/sparse_engine.py``).
 * ``CpuBackend``  -- the plumbing/oracle configuration (BASELINE config 1: CPU + gloo):
   shards live in ``libexb_core`` and ids / rows / grads travel with

@@ -236,7 +236,7 @@ def dump_variable_config(table, reserve_items, optimizer, initializer, include_o
     if include_optimizer:
         doc[oc] = opt
     doc[ic] = ini
-    # B200 addition: pulls never insert, so never-updated rows are regenerated from Philox(seed, variable_id).
+    # addition of this engine: pulls never insert, so never-updated rows are regenerated from Philox(seed, variable_id).
     # The seed therefore has to travel with the checkpoint (the reference loader only warns about unknown keys,
     # Factory.h:64-75); seed 0 (the default) is left out so that default dumps stay byte-identical.
     if seed:
@@ -278,7 +278,7 @@ _ENV_DEFAULTS = {
         "pmem_pool_root_path": "", "cache_size": 1024, "message_compress": "",
         "server_dump_files": 1, "server_concurrency": -1, "recv_timeout": -1, "report_interval": -1,
         "update_early_return": True,
-        # B200 engine additions
+        # additions of this engine
         "hash_table_reserve": 1 << 20, "host_tier_root_path": "", "deterministic": False,
         # HBM accounting (reference: ShardStorageMemory soft / hard limits, pico-ps storage/Storage.h:261-289): MB of
         # device memory the sparse engine of ONE rank may hold (tables + optimizer state + plans + tier caches);

@@ -4,7 +4,7 @@ Reference: ``_get_context()`` / ``Context`` in openembedding/tensorflow/exb.py:1
 the C++ ``WorkerContext`` (openembedding/client/WorkerContext.cpp:7-163): connection to
 the master, storage / variable creation broadcast to all workers, model uuid, barrier.
 
-B200 design: rendezvous and object broadcast ride on ``torch.distributed`` (NCCL group
+Design: rendezvous and object broadcast ride on ``torch.distributed`` (NCCL group
 for GPUs, gloo for the CPU configuration); the data plane is ``backend.CudaBackend``.
 """
 import atexit

@@ -1,6 +1,6 @@
 // exb_core.cpp -- CPU parameter-shard engine + checkpoint shard-file IO, C ABI ("exb_*").
 //
-// Role in the B200 framework: (1) the numerical oracle every CUDA kernel is tested
+// Role in the framework: (1) the numerical oracle every CUDA kernel is tested
 // against, (2) the data path of the CPU/gloo configuration, (3) the native checkpoint
 // reader/writer that speaks the reference's on-disk format bit for bit, (4) the backing
 // store of the host-DRAM overflow tier.

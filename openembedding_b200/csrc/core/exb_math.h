@@ -1,4 +1,4 @@
-// exb_math.h -- host/device math shared by the CPU core and the sm_100a kernels.
+// exb_math.h -- host/device math shared by the CPU core and the sm_90a kernels.
 //
 // One definition of every sparse optimizer and every initializer so that the CPU
 // engine (oracle, gloo path) and the CUDA engine compute the same thing.
@@ -6,7 +6,7 @@
 // Behavioural parity targets (reference, read-only):
 //   optimizers   openembedding/variable/EmbeddingOptimizer.h:49-390
 //   initializers openembedding/variable/EmbeddingInitializer.h:20-93
-// Design differences (deliberate, B200-first):
+// Design differences (deliberate, GPU-first):
 //   * row update is expressed per element (+ a per-row scalar prologue) so a lane
 //     group of a warp can update one row cooperatively with float4 accesses;
 //   * initializers are counter-based (Philox4x32-10 keyed by (seed, variable, row))

@@ -1,13 +1,11 @@
 // bulk_rows.cuh -- asynchronous row movement through shared memory.
 //
-// Measured on B200 (profiles/sparse_path.md): a random 256-byte row in a 16-54 GB table
-// costs 2.5-5 us to fetch (DRAM + TLB miss), so a register-staged gather is purely
-// latency-bound (8 rows in flight per lane group, 25 % occupancy, 8 % of DRAM bandwidth).
-// Two async mechanisms were tried:
-//   * 1-D TMA, one cp.async.bulk (UBLKCP) per row: correct, but the per-SM TMA unit
-//     retires one small copy every ~50-60 cycles -> ~12 us per 384-copy pass (removed);
-//   * cp.async 16-byte (LDGSTS): a warp instruction moves 512 B in ~8 issue cycles, holds
-//     no registers while in flight and queues arbitrarily deep -> the path used below.
+// Random rows of a large table are fetched with DRAM and TLB misses, so a gather that stages
+// rows in registers is bound by how many rows it keeps in flight. Rows therefore move with
+// cp.async 16-byte copies (LDGSTS), which hold no registers while in flight and queue deep;
+// one 1-D TMA copy (cp.async.bulk) per row was the other candidate. The choice was made by
+// measurement on the GPUs the engine was first written for and has not been re-measured
+// on H100.
 // A warp keeps a whole task (32 weight rows, or up to 13 x {weights, state, accumulator}) in
 // flight; peer-mapped (NVLink) addresses take the same path.
 #pragma once
@@ -77,7 +75,7 @@ __device__ __forceinline__ void pull_rows_bulk(const TableDev& T, const float* s
 //   split >= dim: not a split feature (bulk = wstride); else columns [split, dim) go to out[b, off2 ...].
 // LPR (lanes per row of the bulk part, power of two >= bulk / 4) is a template parameter: every loop below has a
 // compile-time trip count and unrolls -- the run-time form executed ~1300 instructions per warp task, and a warp
-// task is one dependent chain (ncu: profiles/r2/pull_plan_ncu.md).
+// task is one dependent chain.
 template <int LPR, class Mid>
 __device__ __forceinline__ void pull_rows_fast_t(const TableDev& T, const float* src, unsigned long long id, int flag,
                                                  int b0, int n_rows, float* __restrict__ out, int io_stride, int off,

@@ -1,5 +1,5 @@
 // cin_kernels.cu -- the interaction (outer product) half of xDeepFM's Compressed Interaction Network, laid out for the
-// tcgen05 GEMM that does the other half (the 1x1 convolution over the H_k x m interaction channels).
+// wgmma GEMM that does the other half (the 1x1 convolution over the H_k x m interaction channels).
 //
 // A CIN layer is  out[b, n, d] = relu( sum_{h, j} W[n, h*m + j] * hid[b, h, d] * x[b, j, d] + bias[n] ).
 // With rows r = (b, d) this is ONE GEMM  out[R, N] = Z[R, C] W^T  with  Z[r, h*m + j] = hid[r, h] * x[r, j],  C = H_k*m.
@@ -125,7 +125,7 @@ int exb_cin_outer(uint64_t hid, int hid_bf16, long long ld_hid, int H, uint64_t 
     if (H > CIN_MAX_H || m > CIN_MAX_M || H < 1 || m < 1) { g_cin_err = "cin_outer: H <= 256, m <= 64"; return -1; }
     if (Kp % 8 || H * m + 1 > Kp || ldz % 8) { g_cin_err = "cin_outer: Kp must be a multiple of 8 and hold H*m + 1 columns"; return -1; }
     int grid = (R + CIN_WARPS - 1) / CIN_WARPS;
-    if (grid > 148 * 16) grid = 148 * 16;
+    if (grid > 132 * 16) grid = 132 * 16;
     cudaError_t e = exb::launch_pdl(exb_cin_outer_kernel, dim3(grid), dim3(CIN_WARPS * 32), 0, (cudaStream_t)stream,
                                     (const void*)hid, hid_bf16, ld_hid, H, (const float*)x, ld_x, m, (__nv_bfloat16*)Z, ldz, Kp, R);
     if (e != cudaSuccess) { g_cin_err = cudaGetErrorString(e); return -1; }
@@ -146,7 +146,7 @@ int exb_cin_outer_bwd(uint64_t dZ, long long ldz, uint64_t hid, int hid_bf16, lo
         attr = smem;
     }
     int grid = (R + CIN_WARPS - 1) / CIN_WARPS;
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > 132 * 8) grid = 132 * 8;
     cudaError_t e = exb::launch_pdl(exb_cin_outer_bwd_kernel, dim3(grid), dim3(CIN_WARPS * 32), smem, (cudaStream_t)stream,
                                     (const __nv_bfloat16*)dZ, ldz, (const void*)hid, hid_bf16, ld_hid, H, (const float*)x, ld_x, m,
                                     (float*)dhid, ld_dhid, (float*)dx, ld_dx, R);

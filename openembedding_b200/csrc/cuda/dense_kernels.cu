@@ -7,7 +7,7 @@
 //             of the small parameters, linear-term gradients of the sparse rows
 //   cachegrad scatter-add of the cached tables' gradient rows
 //   adagrad   tf.keras Adagrad over the flat fp32 parameter buffer + refresh of the bf16
-//             K-major weight copies (W and W^T) consumed by the tcgen05 GEMMs
+//             K-major weight copies (W and W^T) consumed by the wgmma GEMMs
 //   allreduce one-shot / two-shot sum over peer-mapped gradient buffers (NVLink P2P), fused
 //             with nothing else on purpose: it replaces the NCCL call of the reference's
 //             Horovod DistributedOptimizer (K5 in SURVEY 2.5)
@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(256) exb_prep_b_kernel(PrepArgs a) {
 //   rows (and copies them into X32 for the FM gradient), appends dense features / padding /
 //   the ones column, and reduces the linear terms into the per-sample base logit.
 //   Replaces prep A (column per thread, needed only while A0^T was materialised) + prep B
-//   (second pass over X32): 25 + 16 us -> see profiles/dense_path.md.
+//   (second pass over X32).
 __global__ void __launch_bounds__(256) exb_prep_row_kernel(PrepArgs a) {
     exb::pdl_trigger();
     exb::pdl_wait();
@@ -457,7 +457,7 @@ __global__ void __launch_bounds__(256) exb_head_row_kernel(HeadArgs a) {
 // parallel steps), duplicates cost one shared-memory read each instead of a global atomic.
 // Cached tables are the small-vocabulary ones (3..4096 rows): the first version issued one global
 // atomic per (sample, chunk) and serialised on the hot rows. Shared-memory float atomics were
-// tried for the tiniest tables and were 1.5x slower (profiles/dense_path.md).
+// tried for the tiniest tables and were slower.
 // The kernel also produces the cached tables' linear-term gradients (dlogit summed per id).
 #define EXB_CG_MAXDP 128
 __global__ void __launch_bounds__(256) exb_cachegrad_kernel(const float* G32, long long xs, int col0, int Dp,
@@ -521,7 +521,7 @@ __global__ void __launch_bounds__(256) exb_cachegrad_kernel(const float* G32, lo
 
 // ---- dense optimizer step: Adagrad + bf16 weight refresh + gradient clearing in ONE pass ----
 // theta is the flat fp32 parameter buffer; the first `nmat` segments are the MLP weight matrices
-// [R, C] whose bf16 copy Wb [R, C] and transposed copy WTb [C, R] feed the tcgen05 GEMMs of the
+// [R, C] whose bf16 copy Wb [R, C] and transposed copy WTb [C, R] feed the wgmma GEMMs of the
 // next step. A 256-thread CTA (32x8) walks 32x32 tiles: read g/accum/w once, write w/accum, the
 // bf16 tile, the transposed bf16 tile (through shared memory) and zero the gradient, so the
 // step needs no separate memset / Adagrad / 3x refresh launches. Elements outside the matrices
@@ -721,7 +721,7 @@ __global__ void exb_refresh_bf16_kernel(const float* W, __nv_bfloat16* Wb, __nv_
 //   last CTA to finish signals "my stores have landed" | every CTA polls for all peers
 //   Adagrad over the whole (now identical on every rank) gradient, fused behind the wait.
 // Two flag exchanges per call instead of the three barrier kernels + two memcpys of the
-// first version (89 us -> see profiles/). Flags are monotonically increasing epochs.
+// first version. Flags are monotonically increasing epochs.
 struct ArArgs {
     float* buf[8];          // every rank's gradient buffer (peer mapped), index = rank
     unsigned* flags[8];     // every rank's flag array [8]
@@ -739,8 +739,7 @@ __device__ __forceinline__ void ar_signal(const ArArgs& a, unsigned e) {   // th
 }
 // ONE polling thread per CTA reads the whole local flag row (<= 8 words) with two 16-byte loads and
 // backs off between polls: W threads x several hundred CTAs re-reading one L2 line every ~0.5 us
-// saturated its slice -- CTAs noticed a flag up to 14 us after it had been set (per-CTA stamps,
-// profiles/sparse_path.md).
+// saturated its slice -- CTAs noticed a flag many microseconds after it had been set (per-CTA stamps).
 __device__ __forceinline__ bool ar_flags_reached(const unsigned* row, int W, unsigned e) {
     unsigned v[8];
     asm volatile("ld.relaxed.sys.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "l"(row) : "memory");
@@ -817,7 +816,7 @@ __global__ void __launch_bounds__(256) exb_ar_fused_kernel(ArArgs a, DenseOptArg
         // gpu-scope release of the CTA's (peer) stores into the arrival count; the LAST CTA's
         // st.release.sys below is cumulative over everything it acquired through that count, so only
         // one system-scope fence sits on the critical path (a MEMBAR.SYS with NVLink stores in flight
-        // was measured at 15-20 us at 8 GPUs: profiles/sparse_path.md)
+        // costs microseconds at 8 GPUs)
         asm volatile("fence.acq_rel.gpu;" ::: "memory");
         s_last = atomicAdd(a.gcount, 1u) == gridDim.x - 1;
     }
@@ -896,7 +895,7 @@ int exb_cachegrad(uint64_t G32, long long xs, int col0, int Dp, uint64_t ids, in
 }
 int exb_adagrad_flat(uint64_t theta, uint64_t accum, uint64_t grad, long long n, float lr, float eps, uint64_t stream) {
     int grid = (int)((n / 4 + 255) / 256);
-    if (grid > 148 * 4) grid = 148 * 4;
+    if (grid > 132 * 4) grid = 132 * 4;
     if (grid < 1) grid = 1;
     cudaError_t e = exb::launch_pdl(exb_adagrad_flat_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, (float*)theta,
                                     (float*)accum, (const float*)grad, n, lr, eps);
@@ -916,7 +915,7 @@ int exb_dense_opt(const void* args, uint64_t stream) {
     int tiles = 0;
     for (int i = 0; i < o.nmat; ++i) tiles += ((o.mat[i].R + 31) / 32) * ((o.mat[i].C + 31) / 32);
     int grid = tiles > 0 ? tiles : 1;
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > 132 * 8) grid = 132 * 8;
     cudaError_t e = exb::launch_pdl(exb_dense_opt_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, o);
     if (e != cudaSuccess) { g_dense_err = cudaGetErrorString(e); return -1; }
     return 0;
@@ -936,7 +935,7 @@ int exb_allreduce_adagrad(const uint64_t* bufs, const uint64_t* flags, uint64_t 
     DenseOptArgs o;
     memset(&o, 0, sizeof(o));
     if (opt_args) o = *reinterpret_cast<const DenseOptArgs*>(opt_args);
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     // CTAs wait on each other (flag polls, arrival counter): the grid must be resident. Up to 4 CTAs per

@@ -2,8 +2,8 @@
 //
 // The reference registers float AND double tables (openembedding/variable/EmbeddingVariable.cpp:277-278) and its
 // optimizer parity test runs both (test/optimizer_test.py:6-72). The fused fp32 engine (engine.cu) is built around
-// 128-bit fp32 vectors and fp32 atomics; double precision is not a throughput path on Blackwell (the fp64 pipe is
-// vestigial), so fp64 tables get this small, exact engine instead: every row is [weights | optimizer state] in the
+// 128-bit fp32 vectors and fp32 atomics; double precision is not the throughput path of these
+// tables (fp64 runs at a fraction of the fp32 rate and doubles the bytes per row), so fp64 tables get this small, exact engine instead: every row is [weights | optimizer state] in the
 // reference's own layout (EmbeddingOptimizerVariable.h:141), rows live in an open-addressing slab in HBM, and the
 // verbs are the same four as the CPU oracle's (exb_core.cpp: pull / update / get / set) executed by kernels with the
 // SAME shared math header (exb_math.h) in the same per-row order -- the results are bit-identical to the CPU engine.

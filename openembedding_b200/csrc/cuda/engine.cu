@@ -1,4 +1,4 @@
-// engine.cu -- host runtime of the B200 sparse engine + C ABI ("exb_cuda_*").
+// engine.cu -- host runtime of the sparse engine + C ABI ("exb_cuda_*").
 //
 // Owns the HBM slabs of every table shard, the peer mapping (CUDA IPC), the per-plan
 // inbox / combine-map work areas and the launch logic of the fused kernels in
@@ -45,7 +45,7 @@ struct HostTable {
 };
 
 struct Engine {
-    int device = 0, rank = 0, world = 1, sms = 148, max_ctas = 0;
+    int device = 0, rank = 0, world = 1, sms = 132, max_ctas = 0;
     std::vector<HostTable> tables;
     TableDev* d_tables = nullptr;
     size_t d_tables_cap = 0;

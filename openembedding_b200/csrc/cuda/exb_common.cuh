@@ -1,4 +1,4 @@
-// exb_common.cuh -- device-side data model of the B200 sparse engine.
+// exb_common.cuh -- device-side data model of the sparse engine.
 //
 // The reference is a CPU parameter server: worker -> RPC -> server thread -> RPC -> worker
 // (SURVEY 3.2/3.3). Here every rank maps every peer's table slabs, inbox and flag words

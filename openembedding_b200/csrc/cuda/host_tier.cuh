@@ -6,7 +6,7 @@
 // (PmemEmbeddingItemPool.h:133-365), the pull-triggered ASYNC promotion of
 // PmemEmbeddingOptimizerVariable.h:129-192 and the cache budget of PersistManager.h:12-83.
 //
-// B200 mapping (one tier per rank and table):
+// GPU mapping (one tier per rank and table):
 //   PMem pool   -> `hrows`: PINNED host DRAM (cudaHostAlloc), one slab of [weights | optimizer state] rows. The GPU
 //                  reads and writes it directly over PCIe (zero-copy): no CPU thread, no staging copy, no ids.cpu().
 //   pool index  -> `hkeys`: open-addressing id -> host-row index kept in HBM (8 B per host row), so every atomic of the

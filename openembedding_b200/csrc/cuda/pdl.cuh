@@ -1,7 +1,7 @@
 // Programmatic dependent launch (PDL) for the kernels of a training step.
 //
 // A step is ~25 short kernels (3-40 us each); at that size the launch latency, the CTA ramp-up
-// and the setup code of a kernel (barrier init, TMEM allocation, descriptor staging) are a
+// and the setup code of a kernel (barrier init, tensor-map prefetch, descriptor staging) are a
 // visible fraction of its run time. Every hot kernel therefore
 //   * is launched with cudaLaunchAttributeProgrammaticStreamSerialization, so the stream (or
 //     the captured graph edge) lets it start while its predecessor is still draining,

@@ -1,4 +1,4 @@
-// sparse_kernels.cuh -- the two fused sparse hot paths of the engine (sm_100a).
+// sparse_kernels.cuh -- the two fused sparse hot paths of the engine (sm_90a).
 //
 //  exb_pull_kernel        K1+K2+K3 of SURVEY 2.5: bucketize by owner (id % S), one-sided
 //                         peer loads of the rows over NVLink (array: direct address, hash:

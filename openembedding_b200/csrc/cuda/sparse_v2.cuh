@@ -10,7 +10,7 @@
 //   * prefetch: a future batch's pull may be issued early and is parked until batch_id catches up
 //             (exb_ops.cpp:139-175, EmbeddingPullOperator.cpp:117-145, Prefetch.h:11-72).
 //
-// B200 design. A plan owns TWO batch slots (double buffer). A slot is the per-step state:
+// Design. A plan owns TWO batch slots (double buffer). A slot is the per-step state:
 //   per-table open-addressing map  id -> h   (h doubles as the row index of the slot's slabs)
 //   slot_of[f][b]                   h of every lookup of the batch
 //   ulist/ukeys/ucount              unique ids in insertion order
@@ -125,7 +125,7 @@ exb_plan_kernel(const TableDev* __restrict__ tables, PlanDev P, const long long*
 }
 
 // Training pull: the stateless one-pass gather of exb_pull_kernel (every lookup reads its row where it lives --
-// measured on 2 and 8 B200s the step is bound by the NUMBER of dependent phases, not by NVLink bytes, so the
+// on several GPUs the step is bound by the NUMBER of dependent phases, not by NVLink bytes, so the
 // one-pass gather beats the unique-row pull of exb_pull2_kernel) with the batch's de-duplication plan built IN
 // THE SAME LAUNCH and in the shadow of the gather: every warp issues the cp.async loads of its 32 rows, inserts
 // the same 32 ids into the slot's map while the rows are in flight, then waits and writes the rows out. The

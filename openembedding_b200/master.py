@@ -6,7 +6,7 @@ acquire/release_lock, generate_id and the rpc/node/model registries
 (rpc/MasterClient.h:56-160); ``Server`` joins a job as a dedicated PS process
 (openembedding/entry/server.cc:25-60, py_api.cc:164-215).
 
-B200 design: inside one NVSwitch box every rank hosts its own shards in HBM, so training
+Design: inside one NVSwitch box every rank hosts its own shards in HBM, so training
 needs no server process and no data-plane RPC. The control plane keeps the same verbs on top
 of a ``torch.distributed.TCPStore`` (the store server thread plays the master): tree paths
 are store keys, children are tracked in an append-only per-parent index, ephemeral nodes are

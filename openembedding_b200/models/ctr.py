@@ -92,7 +92,7 @@ class FusedEmbeddings(nn.Module):
 
 def _gemm_layers(tc):
     """(Linear, Conv1x1) layer classes: on the CUDA engine every GEMM-shaped op of the eager zoo runs on the
-    hand-written tcgen05 kernel (ops/tc_linear.py); on CPU plain torch"""
+    hand-written wgmma kernel (ops/tc_linear.py); on CPU plain torch"""
     if tc:
         from ..ops.tc_linear import TcConv1x1, TcLinear
         return TcLinear, TcConv1x1
@@ -143,7 +143,7 @@ class CIN(nn.Module):
         B, Fn, D = x.shape
         if self.tc and x.is_cuda:
             # own kernels (ops/cin.py): rows = (sample, embedding column); the interaction tensor is written once as
-            # the bf16 operand of the tcgen05 GEMM, bias + relu in its epilogue; no transposes between layers
+            # the bf16 operand of the wgmma GEMM, bias + relu in its epilogue; no transposes between layers
             from ..ops.cin import cin_layer
             xr = x.transpose(1, 2).reshape(B * D, Fn).contiguous().float()
             hidden, outs = xr, []
@@ -227,7 +227,7 @@ class CTRModel(nn.Module):
             self.cache_emb = nn.Parameter(torch.zeros(off, embedding_dim, device=ctx.device)) if self.has_emb else None
             self.cache_lin = nn.Parameter(torch.zeros(off, 1, device=ctx.device))
         dnn_in = nf * embedding_dim + num_dense
-        # GEMM-shaped layers on the hand-written tcgen05 kernel (bf16 operands) when the model computes in bf16 on CUDA
+        # GEMM-shaped layers on the hand-written wgmma kernel (bf16 operands) when the model computes in bf16 on CUDA
         tc = ctx.device.type == "cuda" and compute_dtype == torch.bfloat16
         self.tc = tc
         Linear, _ = _gemm_layers(tc)

@@ -1,10 +1,10 @@
-"""Fused DeepFM / Wide&Deep training step on hand-written sm_100a kernels only.
+"""Fused DeepFM / Wide&Deep training step on hand-written sm_90a kernels only.
 
 Per step and per GPU (10 launches at world 1, captured in one CUDA graph by ``FusedTrainer``):
 
     pull + plan (peer loads, cp.async)   sparse_v2.cuh / sparse_kernels.cuh   (prefetched in the previous step's tail)
     prep                                 dense_kernels.cu   X32 -> A0 (bf16), FM sums, base logit
-    3x GEMM fwd  (tcgen05, relu, ones)   gemm_tcgen05.cu
+    3x GEMM fwd  (wgmma, relu, ones)     gemm_wgmma.cu
     head         (loss, dlogit, dZ_L)    dense_kernels.cu
     backward chain: 3x dX (relu mask / FM-fused fp32 embedding gradient) + 3x dW (MN-major operands, split-K,
                  TMA reduce-add) as ONE persistent kernel (exb_gemm_chain_kernel)
@@ -272,7 +272,7 @@ class FusedCTR:
         self._opt_args = oa
         self._grad_dirty = False
         # persistent GEMM chains: forward (fwd1 -> ... -> fwdL) and backward (dX / dW of every layer) in ONE launch
-        # each (csrc/cuda/gemm_tcgen05.cu: exb_gemm_chain_kernel). EXB_GEMM_CHAIN=0: one launch per GEMM.
+        # each (csrc/cuda/gemm_wgmma.cu: exb_gemm_chain_kernel). EXB_GEMM_CHAIN=0: one launch per GEMM.
         mode = os.environ.get("EXB_GEMM_CHAIN", "bwd")          # "0" | "bwd" | "1" (forward and backward)
         self.use_chain = mode != "0" and self.mn_major and L <= 4
         self.chain_fwd = self.use_chain and mode == "1"

@@ -1,7 +1,7 @@
 """One Compressed-Interaction-Network layer (xDeepFM) on own kernels: interaction + 1x1 convolution + bias + relu.
 
 ``out[r, n] = relu(sum_{h, j} W[n, h*m + j] * hid[r, h] * x[r, j] + bias[n])`` with rows ``r = (batch, embedding column)``.
-The interaction tensor is written once, directly as the bf16 K-major operand of the tcgen05 GEMM
+The interaction tensor is written once, directly as the bf16 K-major operand of the wgmma GEMM
 (``csrc/cuda/cin_kernels.cu: exb_cin_outer_kernel``; a constant-one column carries the bias), the GEMM applies the relu
 in its epilogue, and the backward folds the GEMM's input gradient back into ``d hid`` / ``d x`` with one warp per row
 (``exb_cin_outer_bwd_kernel``). Everything stays in the ``[B*D, channels]`` layout between layers -- no fp32 interaction

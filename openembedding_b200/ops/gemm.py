@@ -1,4 +1,4 @@
-"""Python face of the hand-written tcgen05 GEMM (``csrc/cuda/gemm_tcgen05.cu``).
+"""Python face of the hand-written wgmma GEMM (``csrc/cuda/gemm_wgmma.cu``).
 
 ``gemm_nt(A, B, ...)`` computes ``A[M,K] @ B[N,K].T`` on bf16 operands with one of the
 fused epilogues. Operands must be K-padded to a multiple of 64 and have leading
@@ -28,6 +28,7 @@ def _lib():
         lib.exb_gemm_bf16_tn.argtypes = [c_uint64, c_longlong, c_uint64, c_longlong, c_int, c_int, c_int, c_uint64,
                                          c_longlong, c_int, c_uint64]
         lib.exb_gemm_last_error.restype = ctypes.c_char_p
+        lib.exb_gemm_timeouts.restype = c_int
         lib.exb_chain_desc_size.restype = c_int
         lib.exb_chain_create.restype = ctypes.c_void_p
         lib.exb_chain_create.argtypes = [ctypes.c_void_p, c_int, c_int]
@@ -41,12 +42,20 @@ def _lib():
     return lib
 
 
+def check():
+    """Synchronise the device and raise if a GEMM kernel launched since the last check gave up waiting on its
+    shared-memory pipeline (its output is then wrong)."""
+    n = _lib().exb_gemm_timeouts()
+    if n != 0:
+        raise RuntimeError("GEMM pipeline: %s" % ("%d barrier waits timed out" % n if n > 0 else "status unreadable"))
+
+
 def _p(t):
     return t.data_ptr() if t is not None else 0
 
 
 class ChainDesc(ctypes.Structure):
-    """one GEMM of a persistent chain (csrc/cuda/gemm_tcgen05.cu: struct ChainDesc)"""
+    """one GEMM of a persistent chain (csrc/cuda/gemm_wgmma.cu: struct ChainDesc)"""
     _fields_ = [("tn", c_int), ("M", c_int), ("N", c_int), ("K", c_int),
                 ("A", c_uint64), ("B", c_uint64), ("out", c_uint64),
                 ("lda", c_longlong), ("ldb", c_longlong), ("ldo", c_longlong),
@@ -106,6 +115,7 @@ class GemmChain:
         code = self.lib.exb_chain_status(self.h)
         if code:
             raise RuntimeError("GEMM chain error %d (GEMM %d timed out waiting for its producer)" % (code, code - 100))
+        check()
 
     def close(self):
         if self.h:

@@ -1,4 +1,4 @@
-"""Python face of the sm_100a sparse engine (``csrc/cuda/engine.cu``).
+"""Python face of the sm_90a sparse engine (``csrc/cuda/engine.cu``).
 
 ``CudaEngine`` owns the table shards of one rank; ``SparsePlan`` is a fused
 multi-table lookup/update plan: ONE ``pull`` launch gathers every feature of a batch
@@ -368,13 +368,13 @@ class SparsePlan:
         self.connected = engine.world == 1
         # v2 ("plan once per step", csrc/cuda/sparse_v2.cuh): ids are de-duplicated once per batch into one of two
         # batch slots; pull moves unique remote rows, push moves pre-reduced rows. EXB_SPARSE_V2=0: v1 kernels.
-        # default: v2 on one GPU (measured 0.236 vs 0.267 ms/step), v1 with more (N=2: 0.319 vs 0.354 ms/step -- the
-        # extra phases of the pre-reduced push cost more than the halved NVLink rows buy; profiles/r2/sparse_v2.md)
+        # default: v2 on one GPU, v1 with more (the extra phases of the pre-reduced push cost more than the halved
+        # NVLink rows buy)
         env = os.environ.get("EXB_SPARSE_V2")
         self.v2 = (env != "0") if env is not None else (engine.world == 1)
         # EXB_PULL2=1: training pulls of world > 1 move UNIQUE remote rows (exb_pull2_kernel: gather unique rows,
-        # grid barrier, expand). Measured slower than the one-pass gather on 2 and 8 B200s (the step is bound by the
-        # number of dependent phases, not by NVLink bytes -- profiles/r2/sparse_v2.md), hence off by default.
+        # grid barrier, expand). It adds dependent phases, and on several GPUs the step is bound by the number of
+        # dependent phases rather than by NVLink bytes, hence off by default.
         self.pull2 = os.environ.get("EXB_PULL2", "0") == "1" and self.feat_split is None
         self._armed = [None, None]       # relative slots (0 current, 1 next): ((ids ptr, n), origin) or None
         engine.plans.append(self)

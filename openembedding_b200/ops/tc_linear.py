@@ -1,14 +1,14 @@
 """``TcLinear`` / ``tc_matmul``: ``torch.nn.Linear`` whose three GEMMs (forward, input gradient, weight gradient) run
-on the hand-written tcgen05 kernel (``csrc/cuda/gemm_tcgen05.cu``) instead of cuBLAS.
+on the hand-written wgmma kernel (``csrc/cuda/gemm_wgmma.cu``) instead of cuBLAS.
 
 Used by the eager model zoo (``models/ctr.py``) for everything that is GEMM-shaped and not covered by the fully fused
 DeepFM / WDL step: the DNN towers of xDeepFM / DCN-v2, the DCN-v2 cross layers (``x0 * (W x + b) + x``) and the CIN's
 1x1 convolutions (a GEMM over the ``H_k x m`` interaction channels, xDeepFM). The reference gets these from
 TensorFlow -> cuBLAS / cuDNN (K6 in SURVEY 2.5).
 
-bf16 operands, fp32 accumulation in TMEM, fp32 master weights / bias / gradients. Operands are padded to the tile
+bf16 operands, fp32 accumulation in registers, fp32 master weights / bias / gradients. Operands are padded to the tile
 geometry (K to a multiple of 64, the batch to a multiple of 64 for the weight-gradient product, which reads the
-batch-major activations as MN-major UMMA operands -- no transposed copies).
+batch-major activations as MN-major wgmma operands -- no transposed copies).
 """
 import torch
 from torch import nn
@@ -73,7 +73,7 @@ class _TcLinearFn(torch.autograd.Function):
 
 
 def tc_linear(x, weight, bias=None):
-    """``x @ weight.T + bias`` on the tcgen05 GEMM; x may have any leading shape"""
+    """``x @ weight.T + bias`` on the wgmma GEMM; x may have any leading shape"""
     lead = x.shape[:-1]
     y = _TcLinearFn.apply(x.reshape(-1, x.shape[-1]), weight, bias)
     return y.reshape(lead + (weight.shape[0],))

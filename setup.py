@@ -1,7 +1,7 @@
 """``pip install .`` / ``python setup.py build_ext --inplace``: compiles the two native libraries IN TREE
-(``openembedding_b200/lib/libexb_core.so`` with g++, ``libexb_cuda.so`` with nvcc for sm_100a) and ships them as
+(``openembedding_b200/lib/libexb_core.so`` with g++, ``libexb_cuda.so`` with nvcc for sm_90a) and ships them as
 package data -- the counterpart of the reference's sdist that compiles its pybind module and TF ops at install
-time (/root/reference/setup.py:19-38). The libraries are also (re)built lazily on first import when stale."""
+time (the reference's setup.py:19-38). The libraries are also (re)built lazily on first import when stale."""
 import os
 import sys
 

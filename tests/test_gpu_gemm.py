@@ -1,8 +1,16 @@
-"""tcgen05 GEMM vs a plain PyTorch fp32 reference of the same op, every fused epilogue."""
+"""wgmma GEMM vs a plain PyTorch fp32 reference of the same op, every fused epilogue."""
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(autouse=True)
+def _no_pipeline_timeouts():
+    """every GEMM launched by a test must have completed its shared-memory pipeline"""
+    yield
+    from openembedding_b200.ops.gemm import check
+    check()
 
 
 def _mk(rows, cols, ld=None, scale=1.0, seed=0):
@@ -79,7 +87,7 @@ def test_dx_fm():
 @pytest.mark.parametrize("M,N,K,splits", [(128, 64, 64, 1), (64, 64, 128, 1), (448, 1728, 4096, 8), (448, 448, 4096, 8),
                                           (100, 72, 256, 2)])
 def test_dw_mn_major(M, N, K, splits):
-    """out = A[K,M]^T @ B[K,N] from batch-major operands (MN-major UMMA tiles, no transposed copies)"""
+    """out = A[K,M]^T @ B[K,N] from batch-major operands (MN-major wgmma tiles, no transposed copies)"""
     from openembedding_b200.ops.gemm import gemm_tn
     ldm, ldn = (M + 7) // 8 * 8, (N + 7) // 8 * 8
     A, B = _mk(K, M, ld=ldm, scale=0.1, seed=11), _mk(K, N, ld=ldn, scale=0.1, seed=12)
@@ -155,7 +163,7 @@ def test_chain_matches_single_launches(M):
 
 @pytest.mark.parametrize("M,K,N", [(256, 100, 40), (1000, 247, 400), (130, 64, 1)])
 def test_tc_linear_matches_torch(M, K, N):
-    """forward, dX, dW, db of TcLinear (tcgen05 GEMMs) vs nn.Linear in fp32"""
+    """forward, dX, dW, db of TcLinear (wgmma GEMMs) vs nn.Linear in fp32"""
     from openembedding_b200.ops.tc_linear import TcLinear
     torch.manual_seed(0)
     ref = torch.nn.Linear(K, N).cuda()
@@ -181,7 +189,7 @@ def test_tc_linear_matches_torch(M, K, N):
 @pytest.mark.parametrize("B,Fn,D,layers,split", [(64, 26, 9, (128, 128), True), (50, 7, 16, (32, 16, 8), True),
                                                  (33, 5, 4, (24,), False)])
 def test_cin_own_kernels_match_torch(B, Fn, D, layers, split):
-    """xDeepFM CIN on own kernels (interaction written as the GEMM operand + tcgen05 GEMM with bias/relu + row-wise
+    """xDeepFM CIN on own kernels (interaction written as the GEMM operand + wgmma GEMM with bias/relu + row-wise
     backward, ops/cin.py) vs the einsum + Conv1d definition in fp32: output and every gradient"""
     from openembedding_b200.models.ctr import CIN
     torch.manual_seed(1)
@@ -235,3 +243,27 @@ def test_cluster_multicast_variant_matches(monkeypatch):
     r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, EXB_GEMM_MC="8"), stdout=subprocess.PIPE,
                        stderr=subprocess.STDOUT, text=True, timeout=300)
     assert "MC_OK" in r.stdout, r.stdout[-2000:]
+
+
+def test_wide_tile_variant_matches():
+    """EXB_GEMM_BN=128: the 128-wide tile (m64n128k16 wgmma, 3-stage ring, two-block MN-major operands) for every
+    epilogue of gemm_nt and for gemm_tn, through the same checks as the default 64-wide tile"""
+    import subprocess, sys, os
+    here = os.path.dirname(os.path.abspath(__file__))
+    code = (
+        "import sys; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
+        "import test_gpu_gemm as T\n"
+        "from openembedding_b200.ops.gemm import check\n"
+        "for shape in [(128, 64, 64), (256, 128, 192), (300, 200, 128), (4096, 448, 448)]:\n"
+        "    T.test_fwd_relu_ones_transposed(*shape)\n"
+        "T.test_dx_mask()\n"
+        "for s in (1, 4):\n"
+        "    T.test_dw_splitk(s)\n"
+        "T.test_dx_fm()\n"
+        "for shape in [(128, 64, 64, 1), (448, 1728, 4096, 8), (100, 200, 256, 2)]:\n"
+        "    T.test_dw_mn_major(*shape)\n"
+        "check()\n"
+        "print('BN128_OK')\n" % (os.path.dirname(here), here))
+    r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, EXB_GEMM_BN="128"), stdout=subprocess.PIPE,
+                       stderr=subprocess.STDOUT, text=True, timeout=300)
+    assert "BN128_OK" in r.stdout, r.stdout[-2000:]

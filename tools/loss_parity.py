@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Loss-trajectory parity: the fused engine (bf16 tcgen05 GEMMs, fp32 tables / master weights) vs the plain-PyTorch
+"""Loss-trajectory parity: the fused engine (bf16 wgmma GEMMs, fp32 tables / master weights) vs the plain-PyTorch
 baseline in FP32 (benchmarks/nccl_baseline.py), SAME initial weights, SAME batches, SAME optimizers.
 
 Answers "does the bf16 dense path train like an fp32 model?" (VERDICT r1, weak #3). Prints one JSON line with the

@@ -233,7 +233,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpi& E, float (&acc)[BN 
         const int row = m_blk * BM + q * 32 + qrow;
         const bool rv = row < E.M;
         // dlogit / S / emb exist only when the tile has FM columns (fm_cols = 0: plain fp32 dX, null pointers)
-        const float dl = (E.mode == EPI_DX_FM && rv && n_blk * BN + 31 < E.fm_cols) ? E.dlogit[row] : 0.f;
+        const float dl = (E.mode == EPI_DX_FM && rv && n_blk * BN < E.fm_cols) ? E.dlogit[row] : 0.f;
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
             const int c = 8 * j + 2 * (l & 3);
@@ -253,7 +253,10 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpi& E, float (&acc)[BN 
 #pragma unroll
                 for (int u = 0; u < 2; ++u)
                     if (!rv || !(mv[u] > 0.f) || n + u == E.ones_col || n + u >= E.N) x[u] = 0.f;
-            } else if (E.mode == EPI_DX_FM && rv && (n | 31) < E.fm_cols) {   // whole 32-column groups, like the layout
+            } else if (E.mode == EPI_DX_FM && rv && n < E.fm_cols) {
+                // per column pair: n is even and fm_cols = nf * Dp a multiple of 4, so n + 1 < fm_cols as well.
+                // fm_cols need not be a multiple of 32 (nf * Dp = 208 at dim 8): the columns of a partial
+                // 32-column group are embedding columns too and need the FM term
                 const float2 e2 = *reinterpret_cast<const float2*>(E.emb + (size_t)row * E.ldemb + n);
                 const float* sb = E.S + (size_t)row * E.D;
                 x[0] += dl * (sb[n % E.D] - e2.x);

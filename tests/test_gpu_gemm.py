@@ -66,22 +66,47 @@ def test_dw_splitk(splits):
     assert torch.allclose(out, ref, atol=5e-2, rtol=2e-2), (out - ref).abs().max()
 
 
+# (F fields, D = padded dim, persistent chain): F * D = 1664 is a multiple of 32; 208, 312, 108 and 340 are not,
+# so their last embedding columns share a 32-column group with plain dX columns
+DX_FM_CASES = [(26, 64, False), (26, 8, False), (26, 12, False), (27, 4, False), (5, 68, False), (26, 8, True)]
+
+
 def test_dx_fm():
-    from openembedding_b200.ops.gemm import EPI_DX_FM, gemm_nt
-    Bsz, N, K, D, F = 256, 1728, 448, 64, 26
+    """fp32 embedding gradient dZ @ W + dlogit * (S - e) on the F * D embedding columns, plain dX after them"""
+    for F, D, chain in DX_FM_CASES:
+        _dx_fm_case(F, D, chain)
+
+
+def _dx_fm_case(F, D, chain):
+    from openembedding_b200.ops import gemm as G
+    case = "F=%d D=%d chain=%s" % (F, D, chain)
+    Bsz, N, K = 256, 1728, 448
     dZ, WT = _mk(Bsz, K, seed=8), _mk(N, K, scale=0.1, seed=9)
     g = torch.Generator(device="cuda").manual_seed(10)
     emb = torch.randn(Bsz, 1800, device="cuda", generator=g)
     S = emb[:, :F * D].reshape(Bsz, F, D).sum(1).contiguous()
     dl = torch.randn(Bsz, device="cuda", generator=g)
     out = torch.zeros(Bsz, 1800, device="cuda")
-    gemm_nt(dZ, WT, Bsz, N, K, out, mode=EPI_DX_FM, dlogit=dl, S=S, emb=emb, fm_cols=F * D, D=D)
+    if chain:
+        c = G.GemmChain([G.chain_nt(dZ, WT, Bsz, N, K, out, mode=G.EPI_DX_FM, dlogit=dl, S=S, emb=emb, fm_cols=F * D,
+                                    D=D)], torch.device("cuda"))
+        c.launch()
+        c.check()
+        c.close()
+    else:
+        G.gemm_nt(dZ, WT, Bsz, N, K, out, mode=G.EPI_DX_FM, dlogit=dl, S=S, emb=emb, fm_cols=F * D, D=D)
     torch.cuda.synchronize()
-    ref = dZ.float() @ WT.float().t()
-    fm = dl[:, None, None] * (S[:, None, :] - emb[:, :F * D].reshape(Bsz, F, D))
+    out = out.double()
+    plain = dZ.double() @ WT.double().t()
+    ref = plain.clone()
+    e64, S64 = emb.double(), S.double()
+    fm = dl.double()[:, None, None] * (S64[:, None, :] - e64[:, :F * D].reshape(Bsz, F, D))
     ref[:, :F * D] += fm.reshape(Bsz, -1)
-    assert torch.allclose(out[:, :N], ref, atol=5e-2, rtol=2e-2), (out[:, :N] - ref).abs().max()
-    assert float(out[:, N:].abs().max()) == 0.0
+    assert torch.allclose(out[:, :N], ref, atol=5e-2, rtol=2e-2), (case, float((out[:, :N] - ref).abs().max()))
+    # the columns after the embedding columns carry plain dX, without an FM term
+    assert torch.allclose(out[:, F * D:N], plain[:, F * D:], atol=5e-2, rtol=2e-2), \
+        (case, float((out[:, F * D:N] - plain[:, F * D:]).abs().max()))
+    assert float(out[:, N:].abs().max()) == 0.0, case
 
 
 @pytest.mark.parametrize("M,N,K,splits", [(128, 64, 64, 1), (64, 64, 128, 1), (448, 1728, 4096, 8), (448, 448, 4096, 8),

@@ -35,6 +35,9 @@ ap.add_argument("--prefetch", action="store_true", help="pinned-host input pipel
 ap.add_argument("--steps", type=int, default=100)
 ap.add_argument("--warmup", type=int, default=10)
 ap.add_argument("--cpu", action="store_true")
+ap.add_argument("--engine", default="auto", choices=["auto", "fused", "eager"],
+                help="fused: FusedCTR + FusedTrainer (WDL / DeepFM / xDeepFM, CUDA); eager: CTRModel + Trainer; "
+                     "auto: fused where it exists")
 ap.add_argument("--profile", default="", help="directory: write a chrome trace of 10 steps after the timed run "
                                                 "(reference: --profile / TensorBoard profile_batch, criteo_deepctr.py:290-293), "
                                                 "the vtimer table and the process RSS")
@@ -56,7 +59,11 @@ for name in models:
         reset_context()
         ctx = get_context()
         dev = ctx.device
-        fused = use_cuda and name.lower() in ("deepfm", "wdl")
+        can_fuse = use_cuda and name.lower() in ("deepfm", "wdl", "xdeepfm") and a.batch_size % 128 == 0
+        if a.engine == "fused" and not can_fuse:
+            raise SystemExit("--engine fused: %s at batch %d has no fused step (CUDA, WDL / DeepFM / xDeepFM, "
+                             "batch %% 128 == 0)" % (name, a.batch_size))
+        fused = can_fuse and a.engine != "eager"
         cache = a.batch_size if a.cache else 0
         if fused:
             from openembedding_b200.models.fused_dense import FusedCTR, FusedTrainer

@@ -526,13 +526,15 @@ __global__ void __launch_bounds__(256) exb_cachegrad_kernel(const float* G32, lo
 // bf16 tile, the transposed bf16 tile (through shared memory) and zero the gradient, so the
 // step needs no separate memset / Adagrad / 3x refresh launches. Elements outside the matrices
 // (output weights, dense-linear weights, bias, cached embedding tables) are updated flat.
+// Up to EXB_OPT_MAX_MATS matrices: the DNN layers, then (xDeepFM) the CIN layer filters.
+constexpr int EXB_OPT_MAX_MATS = 8;
 struct OptMat { long long off; int R, C; __nv_bfloat16* Wb; __nv_bfloat16* WTb; };
 struct DenseOptArgs {
     float* theta; float* accum; float* grad;
     long long n, flat_lo;          // [flat_lo, n) is the flat region (matrices come first)
     float lr, eps;
     int nmat, zero_grad;
-    OptMat mat[4];
+    OptMat mat[EXB_OPT_MAX_MATS];
     // optimizer of the dense parameters (tf.keras semantics, the ones the reference benchmark sweeps:
     // test/benchmark/criteo_deepctr.py --optimizer Adagrad | Adam | Ftrl): 0 adagrad, 1 adam, 2 ftrl
     int kind, _pad;
@@ -912,6 +914,7 @@ int exb_refresh_bf16(uint64_t W, uint64_t Wb, uint64_t WTb, int R, int C, uint64
 // Adagrad + bf16 refresh + gradient clearing of the whole dense parameter buffer in one launch
 int exb_dense_opt(const void* args, uint64_t stream) {
     DenseOptArgs o = *reinterpret_cast<const DenseOptArgs*>(args);
+    if (o.nmat < 0 || o.nmat > EXB_OPT_MAX_MATS) { g_dense_err = "dense_opt: at most 8 weight matrices"; return -1; }
     int tiles = 0;
     for (int i = 0; i < o.nmat; ++i) tiles += ((o.mat[i].R + 31) / 32) * ((o.mat[i].C + 31) / 32);
     int grid = tiles > 0 ? tiles : 1;

@@ -1,4 +1,4 @@
-"""Fused DeepFM / Wide&Deep training step on hand-written sm_90a kernels only.
+"""Fused DeepFM / Wide&Deep / xDeepFM training step on hand-written sm_90a kernels only.
 
 Per step and per GPU (10 launches at world 1, captured in one CUDA graph by ``FusedTrainer``):
 
@@ -15,9 +15,13 @@ Per step and per GPU (10 launches at world 1, captured in one CUDA graph by ``Fu
 No cuBLAS, no NCCL, no torch op on the step. Biases are folded into the GEMMs through a
 constant "ones" column, so a layer is exactly one GEMM in each direction.
 
-Model definition = DeepCTR's DeepFM / WDL as used by the reference benchmark
+Model definition = DeepCTR's DeepFM / WDL / xDeepFM as used by the reference benchmark
 (test/benchmark/criteo_deepctr.py:243-282); see ``models/ctr.py`` for the eager version
 of the same architecture (used as the numerical reference in tests).
+
+xDeepFM adds the CIN branch (csrc/cuda/cin_kernels.cu + the wgmma GEMM), 3 + 6 K launches for K layers:
+gather + K x (interaction operand, GEMM) + pool after prep; after the dX GEMM, K x (dY, dZ GEMM, row-wise
+interaction backward, filter-gradient GEMM) and the fold of the CIN embedding gradient into G32.
 """
 import ctypes
 import os
@@ -50,16 +54,36 @@ class _HeadArgs(ctypes.Structure):
                 ("g_cache_lin", c_void_p), ("B", c_int), ("grad_scale", c_float)]
 
 
+_OPT_MAX_MATS = 8          # csrc/cuda/dense_kernels.cu: EXB_OPT_MAX_MATS (DNN layers + CIN layers)
+
+
 class _OptMat(ctypes.Structure):
     _fields_ = [("off", c_longlong), ("R", c_int), ("C", c_int), ("Wb", c_void_p), ("WTb", c_void_p)]
 
 
 class _DenseOptArgs(ctypes.Structure):
     _fields_ = [("theta", c_void_p), ("accum", c_void_p), ("grad", c_void_p), ("n", c_longlong), ("flat_lo", c_longlong),
-                ("lr", c_float), ("eps", c_float), ("nmat", c_int), ("zero_grad", c_int), ("mat", _OptMat * 4),
+                ("lr", c_float), ("eps", c_float), ("nmat", c_int), ("zero_grad", c_int),
+                ("mat", _OptMat * _OPT_MAX_MATS),
                 ("kind", c_int), ("_pad", c_int), ("accum2", c_void_p), ("step", c_void_p), ("b1", c_float), ("b2", c_float),
                 ("l1", c_float), ("l2", c_float), ("l2s", c_float), ("lrp", c_float), ("beta", c_float),
                 ("c1", c_float), ("c2", c_float)]
+
+
+_CIN_MAX_LAYERS = 8        # csrc/cuda/cin_kernels.cu: CIN_MAX_LAYERS
+
+
+class _CinPoolArgs(ctypes.Structure):
+    _fields_ = [("Y", c_void_p * _CIN_MAX_LAYERS), ("ldy", c_longlong * _CIN_MAX_LAYERS),
+                ("lo", c_int * _CIN_MAX_LAYERS), ("hi", c_int * _CIN_MAX_LAYERS), ("K", c_int), ("T", c_int),
+                ("D", c_int), ("B", c_int), ("wcin", c_void_p), ("p", c_void_p), ("base", c_void_p)]
+
+
+class _CinDyArgs(ctypes.Structure):
+    _fields_ = [("Y", c_void_p), ("ldy", c_longlong), ("N", c_int), ("Np", c_int), ("dir_lo", c_int), ("t0", c_int),
+                ("wcin", c_void_p), ("dhid", c_void_p), ("ld_dhid", c_longlong), ("Hn", c_int), ("D", c_int),
+                ("R", c_int), ("dlogit", c_void_p), ("dY", c_void_p), ("lddy", c_longlong), ("p", c_void_p),
+                ("g_wcin", c_void_p), ("T", c_int), ("B", c_int), ("main_ctas", c_int)]
 
 
 def _r(x, m):
@@ -105,12 +129,59 @@ def _ck(rc, what):
         raise RuntimeError("%s: %s" % (what, _lib().exb_dense_last_error().decode()))
 
 
+def _cin_lib():
+    from ..ops import cin as C
+    lib = C._lib()
+    assert lib.exb_cin_pool_args_size() == ctypes.sizeof(_CinPoolArgs), "CinPoolArgs ABI mismatch"
+    assert lib.exb_cin_dy_args_size() == ctypes.sizeof(_CinDyArgs), "CinDyArgs ABI mismatch"
+    return lib
+
+
+def _cin_ck(rc, what):
+    if rc != 0:
+        raise RuntimeError("%s: %s" % (what, _cin_lib().exb_cin_last_error().decode()))
+
+
+def cin_dims(nf, cin_layers, split_half):
+    """Per-layer sizes of the fused CIN: (H, N, Kp, Np, dir_lo) lists. H[k] channels enter layer k (H[0] = nf),
+    the interaction operand Z_k has C_k = H[k] * nf columns plus the bias column, padded to Kp[k]; the layer has
+    N[k] channels padded to Np[k]; its direct (pooled) channels are [dir_lo[k], N[k]). Raises ValueError for the
+    sizes the CIN kernels cannot run."""
+    layers = [int(n) for n in cin_layers]
+    K = len(layers)
+    if K < 1:
+        raise ValueError("xDeepFM needs at least one CIN layer")
+    if nf > 64:
+        raise ValueError("the CIN kernels take at most 64 fields (got %d)" % nf)
+    H, dir_lo = [nf], []
+    for k, n in enumerate(layers):
+        if n < 1:
+            raise ValueError("CIN layer sizes must be positive: %r" % (layers,))
+        last = k == K - 1
+        if split_half and not last and n % 2:
+            raise ValueError("cin_split_half needs even sizes below the last layer: %r" % (layers,))
+        dir_lo.append(n // 2 if split_half and not last else 0)
+        if not last:
+            h = n // 2 if split_half else n
+            if h > 256:
+                raise ValueError("a CIN layer hands at most 256 channels on (got %d)" % h)
+            H.append(h)
+    for h in H:
+        if _r(h * nf, 8) > 12800:       # exb_cin_outer_bwd stages 8 rows of dZ (bf16) in 200 KB of shared memory
+            raise ValueError("CIN interaction width H * fields = %d is above 12800" % (h * nf))
+    Kp = [_r(H[k] * nf + 1, 64) for k in range(K)]
+    Np = [_r(n, 64) for n in layers]
+    return H, layers, Kp, Np, dir_lo
+
+
 class FusedCTR:
-    """DeepFM (use_fm=True) or Wide&Deep (use_fm=False) with the whole step on own kernels."""
+    """DeepFM (use_fm=True), Wide&Deep or xDeepFM (use_fm=False; xDeepFM adds the CIN branch) with the whole step
+    on own kernels."""
 
     def __init__(self, vocab_sizes, num_dense=13, embedding_dim=64, model="deepfm", batch=4096, hidden=None,
                  sparse_optimizer=None, cache_threshold=0, lr=0.001, initial_accumulator_value=0.1, eps=1e-7,
-                 num_shards=None, dw_splits=8, seed=0, pack_linear=None, dense_optimizer=None):
+                 num_shards=None, dw_splits=8, seed=0, pack_linear=None, dense_optimizer=None,
+                 cin_layers=(128, 128), cin_split_half=True):
         from .ctr import FusedEmbeddings
         ctx = get_context()
         if ctx.device.type != "cuda":
@@ -118,15 +189,25 @@ class FusedCTR:
         assert batch % 128 == 0, "the fused dense path needs batch % 128 == 0"
         self.ctx, self.dev, self.lib = ctx, ctx.device, _lib()
         self.model = model.lower()
-        assert self.model in ("deepfm", "wdl")
+        assert self.model in ("deepfm", "wdl", "xdeepfm")
         self.use_fm = self.model == "deepfm"
         self.B, self.nd, self.D = batch, num_dense, embedding_dim
         self.Dp = _r(embedding_dim, 4)
         self.vocab = list(vocab_sizes)
         self.nf = len(self.vocab)
         if hidden is None:
-            hidden = (400, 400, 400) if self.use_fm else (512, 256, 128, 32)
+            hidden = (512, 256, 128, 32) if self.model == "wdl" else (400, 400, 400)
         self.hidden = list(hidden)
+        # xDeepFM: Compressed Interaction Network over the nf embeddings, rows r = (sample, embedding column)
+        self.cin = self.model == "xdeepfm"
+        self.cin_split_half = bool(cin_split_half)
+        self.cin_layers = []
+        if self.cin:
+            self.cin_H, self.cin_layers, self.cin_Kp, self.cin_Np, self.cin_lo = cin_dims(self.nf, cin_layers,
+                                                                                          self.cin_split_half)
+            if len(self.hidden) + len(self.cin_layers) > _OPT_MAX_MATS:
+                raise ValueError("the fused optimizer kernel takes at most %d weight matrices (DNN + CIN layers)"
+                                 % _OPT_MAX_MATS)
         self.Hp = [_r(h + 1, 64) for h in self.hidden]
         self.lr, self.eps, self.dw_splits = lr, eps, int(os.environ.get("EXB_DW_SPLITS", dw_splits))
         self.cached = [f for f, v in enumerate(self.vocab) if 0 < v < cache_threshold]
@@ -168,7 +249,16 @@ class FusedCTR:
             segs["W%d" % l] = (off, n)
             off = _r(off + n, 4)
         L = len(self.hidden)
-        for name, n in (("wout", self.Hp[-1]), ("wd", max(num_dense, 1)), ("bias", 1)):
+        K = len(self.cin_layers)
+        for k in range(K):          # CIN filters [Np_k, Kp_k], bias in column H_k * nf: refreshed matrices as well
+            n = self.cin_Np[k] * self.cin_Kp[k]
+            segs["C%d" % k] = (off, n)
+            off = _r(off + n, 4)
+        flat = [("wout", self.Hp[-1]), ("wd", max(num_dense, 1)), ("bias", 1)]
+        if self.cin:
+            self.cin_T = sum(n - lo for n, lo in zip(self.cin_layers, self.cin_lo))    # pooled CIN features
+            flat.append(("wcin", self.cin_T))
+        for name, n in flat:
             segs[name] = (off, n)
             off = _r(off + n, 4)
         vc = sum(self.vocab[f] for f in self.cached)
@@ -224,9 +314,17 @@ class FusedCTR:
                                                  * math.sqrt(2.0 / (self.hidden[-1] + 1))).to(dev)
         if num_dense:
             self.view("wd")[:num_dense] = (torch.randn(num_dense, generator=gen) * math.sqrt(2.0 / (num_dense + 1))).to(dev)
+        for k in range(K):          # DeepCTR CIN: glorot-uniform filters (fan_in H_k * nf, fan_out N_k), zero biases
+            C, n = self.cin_H[k] * nf, self.cin_layers[k]
+            lim = math.sqrt(6.0 / (C + n))
+            self.cview(k)[:n, :C] = ((torch.rand(n, C, generator=gen) * 2 - 1) * lim).to(dev)
+        if self.cin:                # exFM_logit = Dense(1, use_bias=False, glorot_normal)
+            self.view("wcin")[:] = (torch.randn(self.cin_T, generator=gen) * math.sqrt(2.0 / (self.cin_T + 1))).to(dev)
         # ---- bf16 K-major weight copies
         self.Wb = [torch.zeros(self.Hp[l], dims[l], dtype=bf16, device=dev) for l in range(L)]
         self.WTb = [torch.zeros(dims[l], self.Hp[l], dtype=bf16, device=dev) for l in range(L)]
+        self.cWb = [torch.zeros(self.cin_Np[k], self.cin_Kp[k], dtype=bf16, device=dev) for k in range(K)]
+        self.cWTb = [torch.zeros(self.cin_Kp[k], self.cin_Np[k], dtype=bf16, device=dev) for k in range(K)]
         # ---- activations
         B = batch
         self.X32 = torch.zeros(B, self.XS, dtype=f32, device=dev)
@@ -254,11 +352,11 @@ class FusedCTR:
         self.mn_major = os.environ.get("EXB_MN_MAJOR", "1") != "0"
         self._s2 = torch.cuda.Stream(device=dev)
         self._ev_fork, self._ev_join, self._ev_plan = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
-        assert L <= 4, "the fused optimizer kernel takes at most 4 weight matrices"
+        assert L + K <= _OPT_MAX_MATS, "the fused optimizer kernel takes at most %d weight matrices" % _OPT_MAX_MATS
         oa = _DenseOptArgs()
         oa.theta, oa.accum, oa.grad = self.theta.data_ptr(), self.accum.data_ptr(), self.gtheta.data_ptr()
         oa.n, oa.flat_lo, oa.lr, oa.eps = self.n_theta, segs["wout"][0], self.lr, float(self.dense_opt.get("epsilon", self.eps))
-        oa.nmat, oa.zero_grad = L, 1
+        oa.nmat, oa.zero_grad = L + K, 1
         d = self.dense_opt
         oa.kind = {"adagrad": 0, "adam": 1, "ftrl": 2}[d["category"]]
         oa.accum2, oa.step = self.accum2.data_ptr(), self.opt_step.data_ptr()
@@ -269,7 +367,12 @@ class FusedCTR:
         for l in range(L):
             oa.mat[l].off, oa.mat[l].R, oa.mat[l].C = segs["W%d" % l][0], self.Hp[l], dims[l]
             oa.mat[l].Wb, oa.mat[l].WTb = self.Wb[l].data_ptr(), self.WTb[l].data_ptr()
+        for k in range(K):
+            oa.mat[L + k].off, oa.mat[L + k].R, oa.mat[L + k].C = segs["C%d" % k][0], self.cin_Np[k], self.cin_Kp[k]
+            oa.mat[L + k].Wb, oa.mat[L + k].WTb = self.cWb[k].data_ptr(), self.cWTb[k].data_ptr()
         self._opt_args = oa
+        if self.cin:
+            self._cin_init_buffers()
         self._grad_dirty = False
         # persistent GEMM chains: forward (fwd1 -> ... -> fwdL) and backward (dX / dW of every layer) in ONE launch
         # each (csrc/cuda/gemm_wgmma.cu: exb_gemm_chain_kernel). EXB_GEMM_CHAIN=0: one launch per GEMM.
@@ -311,6 +414,91 @@ class FusedCTR:
         o, n = self.segs[name]
         return self.gtheta[o:o + n]
 
+    def cview(self, k, grad=False):
+        """CIN layer k's filter matrix [Np_k, Kp_k] (bias in column H_k * nf) in theta, or in gtheta"""
+        return (self.gview if grad else self.view)("C%d" % k).view(self.cin_Np[k], self.cin_Kp[k])
+
+    # ---- xDeepFM: the CIN branch (csrc/cuda/cin_kernels.cu + the wgmma GEMM), every buffer allocated here once
+    def _cin_init_buffers(self):
+        B, D, m, K, dev = self.B, self.D, self.nf, len(self.cin_layers), self.dev
+        f32, bf16 = torch.float32, torch.bfloat16
+        self.cin_lib = _cin_lib()
+        self.cin_R = R = B * D            # rows (sample, embedding column); the pad columns Dp - D are no CIN input
+        H, Kp, Np = self.cin_H, self.cin_Kp, self.cin_Np
+        self.cin_X0 = torch.zeros(R, m, dtype=f32, device=dev)
+        self.cin_Z = [torch.zeros(R, Kp[k], dtype=bf16, device=dev) for k in range(K)]       # interaction operands
+        self.cin_Y = [torch.zeros(R, Np[k], dtype=bf16, device=dev) for k in range(K)]       # layer outputs
+        self.cin_dY = [torch.zeros(R, Np[k], dtype=bf16, device=dev) for k in range(K)]
+        self.cin_dZ = [torch.zeros(R, Kp[k], dtype=bf16, device=dev) for k in range(K)]
+        self.cin_dhid = [torch.zeros(R, H[k], dtype=f32, device=dev) for k in range(K)]
+        self.cin_dx = [torch.zeros(R, m, dtype=f32, device=dev) for k in range(K)]
+        self.cin_p = torch.zeros(B, self.cin_T, dtype=f32, device=dev)                        # pooled features
+        pa = _CinPoolArgs()
+        t0s, t0 = [], 0
+        for k in range(K):
+            pa.Y[k], pa.ldy[k] = self.cin_Y[k].data_ptr(), Np[k]
+            pa.lo[k], pa.hi[k] = self.cin_lo[k], self.cin_layers[k]
+            t0s.append(t0)
+            t0 += self.cin_layers[k] - self.cin_lo[k]
+        pa.K, pa.T, pa.D, pa.B = K, self.cin_T, D, B
+        pa.wcin, pa.p, pa.base = self.view("wcin").data_ptr(), self.cin_p.data_ptr(), self.base.data_ptr()
+        self._cin_pool_args = pa
+        self._cin_dy_args = []
+        for k in range(K):
+            last = k == K - 1
+            a = _CinDyArgs()
+            a.Y, a.ldy, a.N, a.Np = self.cin_Y[k].data_ptr(), Np[k], self.cin_layers[k], Np[k]
+            a.dir_lo, a.t0, a.wcin = self.cin_lo[k], t0s[k], self.view("wcin").data_ptr()
+            a.dhid = 0 if last else self.cin_dhid[k + 1].data_ptr()
+            a.ld_dhid, a.Hn = (0, 0) if last else (H[k + 1], H[k + 1])
+            a.D, a.R, a.dlogit = D, R, self.dlogit.data_ptr()
+            a.dY, a.lddy = self.cin_dY[k].data_ptr(), Np[k]
+            a.p, a.g_wcin = self.cin_p.data_ptr(), self.gview("wcin").data_ptr() if last else 0
+            a.T, a.B = self.cin_T, B
+            self._cin_dy_args.append(a)
+        srcs = [self.cin_dx[0], self.cin_dhid[0]] + self.cin_dx[1:]
+        self._cin_fold_srcs = (ctypes.c_uint64 * len(srcs))(*[t.data_ptr() for t in srcs])
+        # split-K of the filter-gradient GEMMs (K = R rows): about two waves of output tiles
+        self.cin_splits = [max(1, min(R // 1024, 264 // ((Np[k] // 128 + 1) * (Kp[k] // 128 + 1)))) for k in range(K)]
+
+    def _cin_hid(self, k):
+        """(tensor, is_bf16, row stride) of layer k's input: X0 (fp32), then the handed-on channels of Y_{k-1}"""
+        if k == 0:
+            return self.cin_X0, 0, self.nf
+        return self.cin_Y[k - 1], 1, self.cin_Np[k - 1]
+
+    def _cin_forward(self, st):
+        """X0 from X32, Z_k / Y_k of every layer, then p and base += p . w_cin (after prep, before the head)"""
+        lib, B, R, m = self.cin_lib, self.B, self.cin_R, self.nf
+        _cin_ck(lib.exb_cin_gather(self.X32.data_ptr(), self.XS, self.Dp, self.D, m, self.cin_X0.data_ptr(), B, st),
+                "cin_gather")
+        for k in range(len(self.cin_layers)):
+            hid, hb, ld = self._cin_hid(k)
+            Kp, Np = self.cin_Kp[k], self.cin_Np[k]
+            _cin_ck(lib.exb_cin_outer(hid.data_ptr(), hb, ld, self.cin_H[k], self.cin_X0.data_ptr(), m, m,
+                                      self.cin_Z[k].data_ptr(), Kp, Kp, R, st), "cin_outer")
+            G.gemm_nt(self.cin_Z[k], self.cWb[k], R, Np, Kp, self.cin_Y[k], mode=G.EPI_FWD, relu=True, ones_col=-1,
+                      stream=st)
+        _cin_ck(lib.exb_cin_pool(ctypes.byref(self._cin_pool_args), st), "cin_pool")
+
+    def _cin_backward(self, st):
+        """dY / dZ / d hid / d x / filter gradients from the last layer down, g_wcin, then the fold of the embedding
+        gradients into G32 (after the DNN's dX GEMM wrote those columns, before cachegrad and the push)"""
+        lib, B, R, m = self.cin_lib, self.B, self.cin_R, self.nf
+        for k in range(len(self.cin_layers) - 1, -1, -1):
+            Kp, Np = self.cin_Kp[k], self.cin_Np[k]
+            _cin_ck(lib.exb_cin_dy(ctypes.byref(self._cin_dy_args[k]), st), "cin_dy")
+            G.gemm_nt(self.cin_dY[k], self.cWTb[k], R, Kp, Np, self.cin_dZ[k], mode=G.EPI_FWD, relu=False, ones_col=-1,
+                      stream=st)
+            hid, hb, ld = self._cin_hid(k)
+            _cin_ck(lib.exb_cin_outer_bwd(self.cin_dZ[k].data_ptr(), Kp, hid.data_ptr(), hb, ld, self.cin_H[k],
+                                          self.cin_X0.data_ptr(), m, m, self.cin_dhid[k].data_ptr(), self.cin_H[k],
+                                          self.cin_dx[k].data_ptr(), m, R, st), "cin_outer_bwd")
+            G.gemm_tn(self.cin_dY[k], self.cin_Z[k], Np, Kp, R, self.cview(k, grad=True), splits=self.cin_splits[k],
+                      stream=st)
+        _cin_ck(lib.exb_cin_fold(self.G32.data_ptr(), self.XS, self.Dp, self.D, m, B, self._cin_fold_srcs,
+                                 len(self._cin_fold_srcs), st), "cin_fold")
+
     def _st(self):
         return torch.cuda.current_stream(self.dev).cuda_stream
 
@@ -328,6 +516,9 @@ class FusedCTR:
         for l in range(len(self.hidden)):
             _ck(self.lib.exb_refresh_bf16(self.view("W%d" % l).data_ptr(), self.Wb[l].data_ptr(),
                                           self.WTb[l].data_ptr(), self.Hp[l], dims[l], self._st()), "refresh_bf16")
+        for k in range(len(self.cin_layers)):
+            _ck(self.lib.exb_refresh_bf16(self.view("C%d" % k).data_ptr(), self.cWb[k].data_ptr(), self.cWTb[k].data_ptr(),
+                                          self.cin_Np[k], self.cin_Kp[k], self._st()), "refresh_bf16")
 
     # ---- one training step (all launches on the current stream)
     def forward_backward(self, ids, dense, labels, update=True, next_ids=None, pulled=False):
@@ -372,6 +563,9 @@ class FusedCTR:
                           ones_col=self.Hp[l] - 1, outT=self.HT[l] if (l < L - 1 and not tn) else None, stream=st)
                 src = self.H[l]
         self._mark("fwd_gemm")
+        if self.cin:
+            self._cin_forward(st)
+            self._mark("cin_fwd")
         row_head = tn and self.Hp[-1] <= 512       # merged row-wise head; cachegrad then owns the cached linear grads
         ha = _HeadArgs(self.H[-1].data_ptr(), self.Hp[-1], self.Hp[-1] - 1, self.view("wout").data_ptr(),
                        self.base.data_ptr(), labels.data_ptr(), self.dlogit.data_ptr(), self.loss.data_ptr(),
@@ -391,6 +585,9 @@ class FusedCTR:
             G.gemm_nt(self.dZ[0], self.WTb[0], B, self.K0p, self.Hp[0], self.G32, mode=G.EPI_DX_FM, dlogit=self.dlogit,
                       S=self.S, emb=self.X32, fm_cols=self.nf * self.Dp if self.use_fm else 0, D=self.Dp, stream=st)
         self._mark("dx_gemm")
+        if self.cin:
+            self._cin_backward(st)
+            self._mark("cin_bwd")
         forked = update and self.overlap
         if forked:
             cur = torch.cuda.current_stream(self.dev)
@@ -483,6 +680,8 @@ class FusedCTR:
         head = 1 if (self.mn_major and self.Hp[-1] <= 512) else 2
         gemms = (1 if self.chain_fwd else L) + (1 if self.use_chain else 2 * L)   # persistent chains: fwd, bwd
         n = 1 + prep + gemms + head + (1 if self.nc else 0) + 1 + 1      # pull prep GEMMs head cache push optimizer
+        # CIN: gather + pool + fold, per layer outer + GEMM forward, dY + dZ GEMM + outer_bwd + filter-gradient GEMM
+        n += 3 + 6 * len(self.cin_layers) if self.cin else 0
         return n + (1 if self._ar is not None and not self._rider else 0)
 
     # ---- fp32 torch reference of the dense math on the current X32 (tests)
@@ -526,9 +725,35 @@ class FusedCTR:
             h = torch.cat([h[:, :-1], ones], dim=1)
         o, n = self.segs["wout"]
         z = z + h.to(torch.bfloat16).float() @ theta[o:o + n]
+        if self.cin:
+            z = z + self._reference_cin(emb.view(B, nf, Dp)[:, :, :self.D], theta)
         loss = torch.nn.functional.binary_cross_entropy_with_logits(z, labels)
         loss.backward()
         return loss.detach(), {"theta": theta.grad, "emb": emb_leaf.grad, "lin": lin_leaf.grad}
+
+    def _reference_cin(self, x, theta):
+        """CIN(x) . w_cin for ``reference``: the eager zoo's ``models.ctr.CIN`` (plain torch) run on the filters in
+        ``theta``, rounded to bf16 where the kernels round -- Z and W on the way into a layer, Y on the way out (the
+        gradients of Z and Y then arrive rounded too, like the kernels' bf16 dZ and dY). x: [B, nf, D] fp32."""
+        from .ctr import CIN
+        bf16 = torch.bfloat16
+        if getattr(self, "_ref_cin", None) is None:
+            cin = CIN(self.nf, tuple(self.cin_layers), split_half=self.cin_split_half, tc=False).to(self.dev)
+            for conv in cin.convs:
+                conv.register_forward_pre_hook(lambda mod, args: (args[0].to(bf16).float(),))
+                conv.register_forward_hook(lambda mod, args, out: out.to(bf16).float())
+            self._ref_cin = cin
+        params = {}
+        for k, n in enumerate(self.cin_layers):
+            o, sz = self.segs["C%d" % k]
+            W = theta[o:o + sz].view(self.cin_Np[k], self.cin_Kp[k])
+            W = W + (W.to(bf16).float() - W).detach()          # bf16 value, fp32 gradient (the kernels' gW)
+            C = self.cin_H[k] * self.nf
+            params["convs.%d.weight" % k] = W[:n, :C].contiguous().unsqueeze(-1)
+            params["convs.%d.bias" % k] = W[:n, C].contiguous()
+        p = torch.func.functional_call(self._ref_cin, params, (x,))
+        o, n = self.segs["wcin"]
+        return p @ theta[o:o + n]
 
 
 class FusedTrainer:

@@ -30,6 +30,18 @@ def _lib():
         lib.exb_cin_outer_bwd.argtypes = [c_uint64, c_longlong, c_uint64, c_int, c_longlong, c_int, c_uint64, c_longlong, c_int,
                                           c_uint64, c_longlong, c_uint64, c_longlong, c_int, c_uint64]
         lib.exb_cin_last_error.restype = ctypes.c_char_p
+        # the fused xDeepFM step (models/fused_dense.py)
+        lib.exb_cin_gather.restype = c_int
+        lib.exb_cin_gather.argtypes = [c_uint64, c_longlong, c_int, c_int, c_int, c_uint64, c_int, c_uint64]
+        lib.exb_cin_pool.restype = c_int
+        lib.exb_cin_pool.argtypes = [ctypes.c_void_p, c_uint64]
+        lib.exb_cin_pool_args_size.restype = c_int
+        lib.exb_cin_dy.restype = c_int
+        lib.exb_cin_dy.argtypes = [ctypes.c_void_p, c_uint64]
+        lib.exb_cin_dy_args_size.restype = c_int
+        lib.exb_cin_fold.restype = c_int
+        lib.exb_cin_fold.argtypes = [c_uint64, c_longlong, c_int, c_int, c_int, c_int, ctypes.POINTER(c_uint64), c_int,
+                                     c_uint64]
         _proto_done = True
     return lib
 

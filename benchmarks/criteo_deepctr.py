@@ -36,7 +36,7 @@ ap.add_argument("--steps", type=int, default=100)
 ap.add_argument("--warmup", type=int, default=10)
 ap.add_argument("--cpu", action="store_true")
 ap.add_argument("--engine", default="auto", choices=["auto", "fused", "eager"],
-                help="fused: FusedCTR + FusedTrainer (WDL / DeepFM / xDeepFM, CUDA); eager: CTRModel + Trainer; "
+                help="fused: FusedCTR + FusedTrainer (WDL / DeepFM / xDeepFM / DCN, CUDA); eager: CTRModel + Trainer; "
                      "auto: fused where it exists")
 ap.add_argument("--profile", default="", help="directory: write a chrome trace of 10 steps after the timed run "
                                                 "(reference: --profile / TensorBoard profile_batch, criteo_deepctr.py:290-293), "
@@ -59,9 +59,9 @@ for name in models:
         reset_context()
         ctx = get_context()
         dev = ctx.device
-        can_fuse = use_cuda and name.lower() in ("deepfm", "wdl", "xdeepfm") and a.batch_size % 128 == 0
+        can_fuse = use_cuda and name.lower() in ("deepfm", "wdl", "xdeepfm", "dcn") and a.batch_size % 128 == 0
         if a.engine == "fused" and not can_fuse:
-            raise SystemExit("--engine fused: %s at batch %d has no fused step (CUDA, WDL / DeepFM / xDeepFM, "
+            raise SystemExit("--engine fused: %s at batch %d has no fused step (CUDA, WDL / DeepFM / xDeepFM / DCN, "
                              "batch %% 128 == 0)" % (name, a.batch_size))
         fused = can_fuse and a.engine != "eager"
         cache = a.batch_size if a.cache else 0

@@ -30,7 +30,7 @@ ap.add_argument("--embedding_dim", type=int, default=9)
 ap.add_argument("--batch_size", type=int, default=16)
 ap.add_argument("--epochs", type=int, default=3)
 ap.add_argument("--cache", action="store_true", help="replicate tables smaller than the batch (sparse_as_dense)")
-ap.add_argument("--fused", action="store_true", help="whole step on the hand-written kernels (CUDA, DeepFM/WDL/xDeepFM)")
+ap.add_argument("--fused", action="store_true", help="whole step on the hand-written kernels (CUDA, DeepFM/WDL/xDeepFM/DCN)")
 ap.add_argument("--cpu", action="store_true")
 ap.add_argument("--checkpoint", default="")
 ap.add_argument("--load", default="")
@@ -62,8 +62,8 @@ label = torch.tensor(part["label"].values, dtype=torch.float32)
 sparse_opt = {"category": args.optimizer.lower()}
 cache = args.batch_size if args.cache else 0
 if args.fused:
-    if args.model not in ("WDL", "DeepFM", "xDeepFM"):
-        raise SystemExit("--fused: WDL, DeepFM or xDeepFM")
+    if args.model not in ("WDL", "DeepFM", "xDeepFM", "DCN"):
+        raise SystemExit("--fused: WDL, DeepFM, xDeepFM or DCN")
     from openembedding_b200.models.fused_dense import FusedCTR, FusedTrainer
     model = FusedCTR(vocab, embedding_dim=args.embedding_dim, model=args.model.lower(), batch=args.batch_size,
                      sparse_optimizer=sparse_opt, cache_threshold=cache)

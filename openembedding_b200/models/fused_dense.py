@@ -1,4 +1,4 @@
-"""Fused DeepFM / Wide&Deep / xDeepFM training step on hand-written sm_90a kernels only.
+"""Fused DeepFM / Wide&Deep / xDeepFM / DCN-v2 training step on hand-written sm_90a kernels only.
 
 Per step and per GPU (10 launches at world 1, captured in one CUDA graph by ``FusedTrainer``):
 
@@ -16,12 +16,16 @@ No cuBLAS, no NCCL, no torch op on the step. Biases are folded into the GEMMs th
 constant "ones" column, so a layer is exactly one GEMM in each direction.
 
 Model definition = DeepCTR's DeepFM / WDL / xDeepFM as used by the reference benchmark
-(test/benchmark/criteo_deepctr.py:243-282); see ``models/ctr.py`` for the eager version
+(test/benchmark/criteo_deepctr.py:243-282) and the zoo's DCN-v2; see ``models/ctr.py`` for the eager version
 of the same architecture (used as the numerical reference in tests).
 
 xDeepFM adds the CIN branch (csrc/cuda/cin_kernels.cu + the wgmma GEMM), 3 + 6 K launches for K layers:
 gather + K x (interaction operand, GEMM) + pool after prep; after the dX GEMM, K x (dY, dZ GEMM, row-wise
 interaction backward, filter-gradient GEMM) and the fold of the CIN embedding gradient into G32.
+
+DCN-v2 adds the cross network on the A0 layout (csrc/cuda/cross_kernels.cu + the wgmma GEMM), 1 + 5 L launches for
+L layers: L x (U_l GEMM, cross forward) before the head; after the dX GEMM, the top of the cross backward and
+L x (P_l GEMM, weight-gradient GEMM, cross backward), the last of which folds the embedding gradient into G32.
 """
 import ctypes
 import os
@@ -86,6 +90,22 @@ class _CinDyArgs(ctypes.Structure):
                 ("g_wcin", c_void_p), ("T", c_int), ("B", c_int), ("main_ctas", c_int)]
 
 
+class _CrossX0(ctypes.Structure):
+    _fields_ = [("X32", c_void_p), ("xs", c_longlong), ("dense", c_void_p), ("nd", c_int), ("E", c_int), ("Dp", c_int),
+                ("D", c_int), ("K0p", c_int), ("B", c_int)]
+
+
+class _CrossFwdArgs(ctypes.Structure):
+    _fields_ = [("x", _CrossX0), ("U", c_void_p), ("Xin", c_void_p), ("Xf", c_void_p), ("Xb", c_void_p),
+                ("wcross", c_void_p), ("base", c_void_p)]
+
+
+class _CrossBwdArgs(ctypes.Structure):
+    _fields_ = [("x", _CrossX0), ("dlogit", c_void_p), ("wcross", c_void_p), ("gin", c_void_p), ("P", c_void_p),
+                ("gout", c_void_p), ("U", c_void_p), ("dU", c_void_p), ("gx0", c_void_p), ("G32", c_void_p),
+                ("XfL", c_void_p), ("g_wcross", c_void_p), ("main_ctas", c_int)]
+
+
 def _r(x, m):
     return (x + m - 1) // m * m
 
@@ -142,6 +162,35 @@ def _cin_ck(rc, what):
         raise RuntimeError("%s: %s" % (what, _cin_lib().exb_cin_last_error().decode()))
 
 
+_cross_proto = False
+
+
+def _cross_lib():
+    global _cross_proto
+    lib = _native.cuda()
+    if not _cross_proto:
+        for fn in (lib.exb_cross_fwd, lib.exb_cross_bwd_top, lib.exb_cross_bwd):
+            fn.restype = c_int
+            fn.argtypes = [c_void_p, ctypes.c_uint64]
+        lib.exb_cross_last_error.restype = ctypes.c_char_p
+        assert lib.exb_cross_fwd_args_size() == ctypes.sizeof(_CrossFwdArgs), "CrossFwdArgs ABI mismatch"
+        assert lib.exb_cross_bwd_args_size() == ctypes.sizeof(_CrossBwdArgs), "CrossBwdArgs ABI mismatch"
+        _cross_proto = True
+    return lib
+
+
+def _cross_ck(rc, what):
+    if rc != 0:
+        raise RuntimeError("%s: %s" % (what, _cross_lib().exb_cross_last_error().decode()))
+
+
+def cross_cols(nf, D, Dp, nd):
+    """Columns of the A0 layout [nf*Dp embedding | nd dense | pad | ones] that hold DCN-v2's input
+    x = [emb (nf*D) | dense (nd)], in the order of x: field j's embedding column d < D is column j*Dp + d, the
+    dense features follow at nf*Dp."""
+    return [j * Dp + d for j in range(nf) for d in range(D)] + [nf * Dp + i for i in range(nd)]
+
+
 def cin_dims(nf, cin_layers, split_half):
     """Per-layer sizes of the fused CIN: (H, N, Kp, Np, dir_lo) lists. H[k] channels enter layer k (H[0] = nf),
     the interaction operand Z_k has C_k = H[k] * nf columns plus the bias column, padded to Kp[k]; the layer has
@@ -175,13 +224,13 @@ def cin_dims(nf, cin_layers, split_half):
 
 
 class FusedCTR:
-    """DeepFM (use_fm=True), Wide&Deep or xDeepFM (use_fm=False; xDeepFM adds the CIN branch) with the whole step
-    on own kernels."""
+    """DeepFM (use_fm=True), Wide&Deep, xDeepFM or DCN-v2 (use_fm=False; xDeepFM adds the CIN branch, DCN-v2 the
+    cross network) with the whole step on own kernels."""
 
     def __init__(self, vocab_sizes, num_dense=13, embedding_dim=64, model="deepfm", batch=4096, hidden=None,
                  sparse_optimizer=None, cache_threshold=0, lr=0.001, initial_accumulator_value=0.1, eps=1e-7,
                  num_shards=None, dw_splits=8, seed=0, pack_linear=None, dense_optimizer=None,
-                 cin_layers=(128, 128), cin_split_half=True):
+                 cin_layers=(128, 128), cin_split_half=True, cross_layers=3):
         from .ctr import FusedEmbeddings
         ctx = get_context()
         if ctx.device.type != "cuda":
@@ -189,7 +238,7 @@ class FusedCTR:
         assert batch % 128 == 0, "the fused dense path needs batch % 128 == 0"
         self.ctx, self.dev, self.lib = ctx, ctx.device, _lib()
         self.model = model.lower()
-        assert self.model in ("deepfm", "wdl", "xdeepfm")
+        assert self.model in ("deepfm", "wdl", "xdeepfm", "dcn")
         self.use_fm = self.model == "deepfm"
         self.B, self.nd, self.D = batch, num_dense, embedding_dim
         self.Dp = _r(embedding_dim, 4)
@@ -207,6 +256,15 @@ class FusedCTR:
                                                                                           self.cin_split_half)
             if len(self.hidden) + len(self.cin_layers) > _OPT_MAX_MATS:
                 raise ValueError("the fused optimizer kernel takes at most %d weight matrices (DNN + CIN layers)"
+                                 % _OPT_MAX_MATS)
+        # DCN-v2: cross network x_{l+1} = x0 * (W_l x_l + b_l) + x_l on the A0 layout, one [K0p, K0p] matrix per layer
+        self.dcn = self.model == "dcn"
+        self.cross_layers = int(cross_layers) if self.dcn else 0
+        if self.dcn:
+            if self.cross_layers < 1:
+                raise ValueError("DCN-v2 needs at least one cross layer (got %d)" % self.cross_layers)
+            if len(self.hidden) + self.cross_layers > _OPT_MAX_MATS:
+                raise ValueError("the fused optimizer kernel takes at most %d weight matrices (DNN + cross layers)"
                                  % _OPT_MAX_MATS)
         self.Hp = [_r(h + 1, 64) for h in self.hidden]
         self.lr, self.eps, self.dw_splits = lr, eps, int(os.environ.get("EXB_DW_SPLITS", dw_splits))
@@ -254,10 +312,16 @@ class FusedCTR:
             n = self.cin_Np[k] * self.cin_Kp[k]
             segs["C%d" % k] = (off, n)
             off = _r(off + n, 4)
+        Lc = self.cross_layers
+        for l in range(Lc):         # cross matrices [K0p, K0p], bias in the ones column: refreshed matrices as well
+            segs["X%d" % l] = (off, self.K0p * self.K0p)
+            off = _r(off + self.K0p * self.K0p, 4)
         flat = [("wout", self.Hp[-1]), ("wd", max(num_dense, 1)), ("bias", 1)]
         if self.cin:
             self.cin_T = sum(n - lo for n, lo in zip(self.cin_layers, self.cin_lo))    # pooled CIN features
             flat.append(("wcin", self.cin_T))
+        if self.dcn:
+            flat.append(("wcross", self.K0p))        # x_L's output weights, zero outside the real columns
         for name, n in flat:
             segs[name] = (off, n)
             off = _r(off + n, 4)
@@ -310,10 +374,19 @@ class FusedCTR:
                 m[:, embedding_dim:] = 0
                 blk[:, :nf * Dp] *= m.reshape(-1)
             W[:h_out, :real_in] = blk.to(dev)
-        self.view("wout")[: self.hidden[-1]] = (torch.randn(self.hidden[-1], generator=gen)
-                                                 * math.sqrt(2.0 / (self.hidden[-1] + 1))).to(dev)
+        # DCN-v2: w_cross and wout are one Dense(1) over [x_L | h_dnn] (glorot normal over the concatenation)
+        self.cross_n = nf * embedding_dim + num_dense if self.dcn else 0
+        std_out = math.sqrt(2.0 / (self.hidden[-1] + self.cross_n + 1))
+        self.view("wout")[: self.hidden[-1]] = (torch.randn(self.hidden[-1], generator=gen) * std_out).to(dev)
         if num_dense:
             self.view("wd")[:num_dense] = (torch.randn(num_dense, generator=gen) * math.sqrt(2.0 / (num_dense + 1))).to(dev)
+        if self.dcn:                # DeepCTR CrossNet (matrix): glorot-normal kernels over the real block, zero biases
+            self.cross_real = torch.tensor(cross_cols(nf, embedding_dim, Dp, num_dense), dtype=torch.long, device=dev)
+            n = self.cross_n
+            self.view("wcross")[self.cross_real] = (torch.randn(n, generator=gen) * std_out).to(dev)
+            for l in range(Lc):
+                blk = torch.randn(n, n, generator=gen) * math.sqrt(2.0 / (n + n))
+                self.xview(l)[self.cross_real[:, None], self.cross_real[None, :]] = blk.to(dev)
         for k in range(K):          # DeepCTR CIN: glorot-uniform filters (fan_in H_k * nf, fan_out N_k), zero biases
             C, n = self.cin_H[k] * nf, self.cin_layers[k]
             lim = math.sqrt(6.0 / (C + n))
@@ -325,6 +398,8 @@ class FusedCTR:
         self.WTb = [torch.zeros(dims[l], self.Hp[l], dtype=bf16, device=dev) for l in range(L)]
         self.cWb = [torch.zeros(self.cin_Np[k], self.cin_Kp[k], dtype=bf16, device=dev) for k in range(K)]
         self.cWTb = [torch.zeros(self.cin_Kp[k], self.cin_Np[k], dtype=bf16, device=dev) for k in range(K)]
+        self.xWb = [torch.zeros(self.K0p, self.K0p, dtype=bf16, device=dev) for l in range(Lc)]
+        self.xWTb = [torch.zeros(self.K0p, self.K0p, dtype=bf16, device=dev) for l in range(Lc)]
         # ---- activations
         B = batch
         self.X32 = torch.zeros(B, self.XS, dtype=f32, device=dev)
@@ -352,11 +427,11 @@ class FusedCTR:
         self.mn_major = os.environ.get("EXB_MN_MAJOR", "1") != "0"
         self._s2 = torch.cuda.Stream(device=dev)
         self._ev_fork, self._ev_join, self._ev_plan = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
-        assert L + K <= _OPT_MAX_MATS, "the fused optimizer kernel takes at most %d weight matrices" % _OPT_MAX_MATS
+        assert L + K + Lc <= _OPT_MAX_MATS, "the fused optimizer kernel takes at most %d weight matrices" % _OPT_MAX_MATS
         oa = _DenseOptArgs()
         oa.theta, oa.accum, oa.grad = self.theta.data_ptr(), self.accum.data_ptr(), self.gtheta.data_ptr()
         oa.n, oa.flat_lo, oa.lr, oa.eps = self.n_theta, segs["wout"][0], self.lr, float(self.dense_opt.get("epsilon", self.eps))
-        oa.nmat, oa.zero_grad = L + K, 1
+        oa.nmat, oa.zero_grad = L + K + Lc, 1
         d = self.dense_opt
         oa.kind = {"adagrad": 0, "adam": 1, "ftrl": 2}[d["category"]]
         oa.accum2, oa.step = self.accum2.data_ptr(), self.opt_step.data_ptr()
@@ -370,9 +445,15 @@ class FusedCTR:
         for k in range(K):
             oa.mat[L + k].off, oa.mat[L + k].R, oa.mat[L + k].C = segs["C%d" % k][0], self.cin_Np[k], self.cin_Kp[k]
             oa.mat[L + k].Wb, oa.mat[L + k].WTb = self.cWb[k].data_ptr(), self.cWTb[k].data_ptr()
+        for l in range(Lc):
+            i = L + K + l
+            oa.mat[i].off, oa.mat[i].R, oa.mat[i].C = segs["X%d" % l][0], self.K0p, self.K0p
+            oa.mat[i].Wb, oa.mat[i].WTb = self.xWb[l].data_ptr(), self.xWTb[l].data_ptr()
         self._opt_args = oa
         if self.cin:
             self._cin_init_buffers()
+        if self.dcn:
+            self._cross_init_buffers()
         self._grad_dirty = False
         # persistent GEMM chains: forward (fwd1 -> ... -> fwdL) and backward (dX / dW of every layer) in ONE launch
         # each (csrc/cuda/gemm_wgmma.cu: exb_gemm_chain_kernel). EXB_GEMM_CHAIN=0: one launch per GEMM.
@@ -417,6 +498,10 @@ class FusedCTR:
     def cview(self, k, grad=False):
         """CIN layer k's filter matrix [Np_k, Kp_k] (bias in column H_k * nf) in theta, or in gtheta"""
         return (self.gview if grad else self.view)("C%d" % k).view(self.cin_Np[k], self.cin_Kp[k])
+
+    def xview(self, l, grad=False):
+        """cross layer l's matrix [K0p, K0p] (out, in; bias in the ones column K0p - 1) in theta, or in gtheta"""
+        return (self.gview if grad else self.view)("X%d" % l).view(self.K0p, self.K0p)
 
     # ---- xDeepFM: the CIN branch (csrc/cuda/cin_kernels.cu + the wgmma GEMM), every buffer allocated here once
     def _cin_init_buffers(self):
@@ -499,6 +584,71 @@ class FusedCTR:
         _cin_ck(lib.exb_cin_fold(self.G32.data_ptr(), self.XS, self.Dp, self.D, m, B, self._cin_fold_srcs,
                                  len(self._cin_fold_srcs), st), "cin_fold")
 
+    # ---- DCN-v2: the cross network (csrc/cuda/cross_kernels.cu + the wgmma GEMM), every buffer allocated here once
+    def _cross_init_buffers(self):
+        B, K0p, Lc, dev = self.B, self.K0p, self.cross_layers, self.dev
+        f32, bf16 = torch.float32, torch.bfloat16
+        self.cross_lib = _cross_lib()
+        self.cross_U = [torch.zeros(B, K0p, dtype=f32, device=dev) for _ in range(Lc)]        # U_l = x_l W_l^T
+        self.cross_Xf = [torch.zeros(B, K0p, dtype=f32, device=dev) for _ in range(Lc)]       # x_{l+1}
+        self.cross_Xb = [torch.zeros(B, K0p, dtype=bf16, device=dev) for _ in range(Lc - 1)]  # bf16 x_{l+1} (GEMM A)
+        self.cross_g = [torch.zeros(B, K0p, dtype=f32, device=dev) for _ in range(2)]         # g_l in cross_g[l % 2]
+        self.cross_gx0 = torch.zeros(B, K0p, dtype=f32, device=dev)
+        self.cross_P = torch.zeros(B, K0p, dtype=f32, device=dev)                             # P_l = dU_l W_l
+        self.cross_dU = torch.zeros(B, K0p, dtype=bf16, device=dev)
+        p = lambda t: t.data_ptr() if t is not None else 0
+
+        def x0():
+            return _CrossX0(self.X32.data_ptr(), self.XS, 0, self.nd, self.nf * self.Dp, self.Dp, self.D, K0p, B)
+        wcross = self.view("wcross").data_ptr()
+        self._cross_fwd_args = []
+        for l in range(Lc):
+            last = l == Lc - 1
+            self._cross_fwd_args.append(_CrossFwdArgs(
+                x0(), p(self.cross_U[l]), p(self.cross_Xf[l - 1]) if l else 0, p(self.cross_Xf[l]),
+                0 if last else p(self.cross_Xb[l]), wcross, p(self.base) if last else 0))
+        a = _CrossBwdArgs()
+        a.x, a.dlogit, a.wcross, a.gout = x0(), p(self.dlogit), wcross, p(self.cross_g[Lc % 2])
+        a.U, a.dU, a.gx0 = p(self.cross_U[Lc - 1]), p(self.cross_dU), p(self.cross_gx0)
+        a.XfL, a.g_wcross = p(self.cross_Xf[Lc - 1]), self.gview("wcross").data_ptr()
+        self._cross_top_args = a
+        self._cross_bwd_args = []
+        for l in range(Lc):
+            a = _CrossBwdArgs()
+            a.x, a.gin, a.P, a.gx0 = x0(), p(self.cross_g[(l + 1) % 2]), p(self.cross_P), p(self.cross_gx0)
+            if l:
+                a.gout, a.U, a.dU = p(self.cross_g[l % 2]), p(self.cross_U[l - 1]), p(self.cross_dU)
+            else:
+                a.G32 = p(self.G32)
+            self._cross_bwd_args.append(a)
+        # split-K of the weight-gradient GEMMs (K = batch): about two waves of 128 x 128 output tiles
+        self.cross_splits = max(1, min(B // 1024, 264 // (K0p // 128 + 1) ** 2))
+
+    def _cross_forward(self, st, dense):
+        """U_l and x_{l+1} of every layer, then base += x_L . w_cross (after the forward GEMMs, before the head)"""
+        lib, B, K0p = self.cross_lib, self.B, self.K0p
+        for l in range(self.cross_layers):
+            src = self.A0 if l == 0 else self.cross_Xb[l - 1]
+            G.gemm_nt(src, self.xWb[l], B, K0p, K0p, self.cross_U[l], mode=G.EPI_DX_FM, fm_cols=0, stream=st)
+            a = self._cross_fwd_args[l]
+            a.x.dense = dense.data_ptr()
+            _cross_ck(lib.exb_cross_fwd(ctypes.byref(a), st), "cross_fwd")
+
+    def _cross_backward(self, st, dense):
+        """g_L, then per layer from the last: P_l, the weight gradient, g_l / dU_{l-1} / gx0, and at layer 0 the fold
+        of the cross network's input gradient into G32 (after the DNN's dX GEMM wrote those columns, before cachegrad
+        and the push)"""
+        lib, B, K0p = self.cross_lib, self.B, self.K0p
+        self._cross_top_args.x.dense = dense.data_ptr()
+        _cross_ck(lib.exb_cross_bwd_top(ctypes.byref(self._cross_top_args), st), "cross_bwd_top")
+        for l in range(self.cross_layers - 1, -1, -1):
+            G.gemm_nt(self.cross_dU, self.xWTb[l], B, K0p, K0p, self.cross_P, mode=G.EPI_DX_FM, fm_cols=0, stream=st)
+            G.gemm_tn(self.cross_dU, self.A0 if l == 0 else self.cross_Xb[l - 1], K0p, K0p, B, self.xview(l, grad=True),
+                      splits=self.cross_splits, stream=st)
+            a = self._cross_bwd_args[l]
+            a.x.dense = dense.data_ptr()
+            _cross_ck(lib.exb_cross_bwd(ctypes.byref(a), st), "cross_bwd")
+
     def _st(self):
         return torch.cuda.current_stream(self.dev).cuda_stream
 
@@ -519,6 +669,9 @@ class FusedCTR:
         for k in range(len(self.cin_layers)):
             _ck(self.lib.exb_refresh_bf16(self.view("C%d" % k).data_ptr(), self.cWb[k].data_ptr(), self.cWTb[k].data_ptr(),
                                           self.cin_Np[k], self.cin_Kp[k], self._st()), "refresh_bf16")
+        for l in range(self.cross_layers):
+            _ck(self.lib.exb_refresh_bf16(self.view("X%d" % l).data_ptr(), self.xWb[l].data_ptr(), self.xWTb[l].data_ptr(),
+                                          self.K0p, self.K0p, self._st()), "refresh_bf16")
 
     # ---- one training step (all launches on the current stream)
     def forward_backward(self, ids, dense, labels, update=True, next_ids=None, pulled=False):
@@ -566,6 +719,9 @@ class FusedCTR:
         if self.cin:
             self._cin_forward(st)
             self._mark("cin_fwd")
+        if self.dcn:
+            self._cross_forward(st, dense)
+            self._mark("cross_fwd")
         row_head = tn and self.Hp[-1] <= 512       # merged row-wise head; cachegrad then owns the cached linear grads
         ha = _HeadArgs(self.H[-1].data_ptr(), self.Hp[-1], self.Hp[-1] - 1, self.view("wout").data_ptr(),
                        self.base.data_ptr(), labels.data_ptr(), self.dlogit.data_ptr(), self.loss.data_ptr(),
@@ -588,6 +744,9 @@ class FusedCTR:
         if self.cin:
             self._cin_backward(st)
             self._mark("cin_bwd")
+        if self.dcn:
+            self._cross_backward(st, dense)
+            self._mark("cross_bwd")
         forked = update and self.overlap
         if forked:
             cur = torch.cuda.current_stream(self.dev)
@@ -682,6 +841,8 @@ class FusedCTR:
         n = 1 + prep + gemms + head + (1 if self.nc else 0) + 1 + 1      # pull prep GEMMs head cache push optimizer
         # CIN: gather + pool + fold, per layer outer + GEMM forward, dY + dZ GEMM + outer_bwd + filter-gradient GEMM
         n += 3 + 6 * len(self.cin_layers) if self.cin else 0
+        # DCN-v2: per layer GEMM + cross forward; backward top, per layer P GEMM + weight-gradient GEMM + cross backward
+        n += 1 + 5 * self.cross_layers if self.dcn else 0
         return n + (1 if self._ar is not None and not self._rider else 0)
 
     # ---- fp32 torch reference of the dense math on the current X32 (tests)
@@ -727,7 +888,9 @@ class FusedCTR:
         z = z + h.to(torch.bfloat16).float() @ theta[o:o + n]
         if self.cin:
             z = z + self._reference_cin(emb.view(B, nf, Dp)[:, :, :self.D], theta)
-        loss = torch.nn.functional.binary_cross_entropy_with_logits(z, labels)
+        if self.dcn:
+            z = z + self._reference_cross(torch.cat([emb.view(B, nf, Dp)[:, :, :self.D].reshape(B, -1), dense], 1), theta)
+        loss =torch.nn.functional.binary_cross_entropy_with_logits(z, labels)
         loss.backward()
         return loss.detach(), {"theta": theta.grad, "emb": emb_leaf.grad, "lin": lin_leaf.grad}
 
@@ -754,6 +917,35 @@ class FusedCTR:
         p = torch.func.functional_call(self._ref_cin, params, (x,))
         o, n = self.segs["wcin"]
         return p @ theta[o:o + n]
+
+    def _reference_cross(self, x, theta):
+        """CrossNetV2(x) . w_cross for ``reference``: the eager zoo's ``models.ctr.CrossNetV2`` (plain torch) run on the
+        cross matrices in ``theta``, rounded to bf16 where the kernels round -- x_l and W_l (bias included) on the way
+        into a layer's GEMM with an fp32 gradient passed straight through, and the gradient of U_l (the kernels' bf16
+        dU). U_l itself stays fp32. x: [B, nf*D + nd] fp32."""
+        from .ctr import CrossNetV2
+        bf16 = torch.bfloat16
+        st = lambda t: t + (t.to(bf16).float() - t).detach()        # bf16 value, fp32 gradient
+
+        def round_grad(mod, args, out):
+            out.register_hook(lambda g: g.to(bf16).float())
+
+        if getattr(self, "_ref_cross", None) is None:
+            net = CrossNetV2(self.cross_n, self.cross_layers, tc=False).to(self.dev)
+            for lin in net.w:
+                lin.register_forward_pre_hook(lambda mod, args: (st(args[0]),))
+                lin.register_forward_hook(round_grad)
+            self._ref_cross = net
+        cols, ones = self.cross_real, self.K0p - 1
+        params = {}
+        for l in range(self.cross_layers):
+            o, sz = self.segs["X%d" % l]
+            W = st(theta[o:o + sz].view(self.K0p, self.K0p))
+            params["w.%d.weight" % l] = W[cols[:, None], cols[None, :]]
+            params["w.%d.bias" % l] = W[cols, ones]
+        xL = torch.func.functional_call(self._ref_cross, params, (x,))
+        o, n = self.segs["wcross"]
+        return xL @ theta[o:o + n][cols]
 
 
 class FusedTrainer:

@@ -31,6 +31,8 @@ ap.add_argument("--batch_size", type=int, default=16)
 ap.add_argument("--epochs", type=int, default=3)
 ap.add_argument("--cache", action="store_true", help="replicate tables smaller than the batch (sparse_as_dense)")
 ap.add_argument("--fused", action="store_true", help="whole step on the hand-written kernels (CUDA, DeepFM/WDL/xDeepFM/DCN)")
+ap.add_argument("--validation_batches", type=int, default=0,
+                help="with --fused: hold out the last N batches of each rank, print val_auc / val_logloss per epoch")
 ap.add_argument("--cpu", action="store_true")
 ap.add_argument("--checkpoint", default="")
 ap.add_argument("--load", default="")
@@ -59,6 +61,13 @@ ids = torch.tensor(part[["C%d" % i for i in range(1, 27)]].values, dtype=torch.i
 dense = torch.tensor(part[["I%d" % i for i in range(1, 14)]].values, dtype=torch.float32)
 label = torch.tensor(part["label"].values, dtype=torch.float32)
 
+if args.validation_batches and not args.fused:
+    raise SystemExit("--validation_batches: evaluation runs on the fused step (--fused)")
+n_val = args.validation_batches * args.batch_size
+if n_val >= n:
+    raise SystemExit("--validation_batches %d leaves no training batch" % args.validation_batches)
+n_train = n - n_val
+
 sparse_opt = {"category": args.optimizer.lower()}
 cache = args.batch_size if args.cache else 0
 if args.fused:
@@ -77,13 +86,23 @@ if args.load:
     embed.load_server_model(model, args.load)
 for epoch in range(args.epochs):
     tot, cnt = 0.0, 0
-    for i in range(0, n, args.batch_size):
+    for i in range(0, n_train, args.batch_size):
         sl = slice(i, i + args.batch_size)
         loss = trainer.step(ids[sl].contiguous().to(ctx.device), dense[sl].to(ctx.device), label[sl].to(ctx.device))
         tot += float(loss)
         cnt += 1
     if ctx.rank == 0:
         print("epoch %d loss %.4f" % (epoch + 1, tot / max(cnt, 1)))
+    if n_val:
+        from openembedding_b200.models.metrics import BinaryMetrics
+        metrics = BinaryMetrics()          # tf.keras.metrics.AUC(): 200 thresholds
+        for i in range(n_train, n, args.batch_size):
+            sl = slice(i, i + args.batch_size)
+            trainer.evaluate(ids[sl].contiguous().to(ctx.device), dense[sl].to(ctx.device), label[sl].to(ctx.device),
+                             metrics)
+        r = metrics.result()                # all ranks: the counters are summed over them
+        if ctx.rank == 0:
+            print("epoch %d val_auc %.4f val_logloss %.4f" % (epoch + 1, r["auc"], r["logloss"]))
     if args.checkpoint:
         embed.save_server_model(model, args.checkpoint + str(epoch + 1))          # include optimizer
 if args.save:

@@ -5,6 +5,7 @@
 //             are gathered here
 //   head      final dot with w_out, sigmoid, BCE loss, dlogit, dZ_last (+ transpose), gradients
 //             of the small parameters, linear-term gradients of the sparse rows
+//   predict   evaluation head: final dot with w_out, logits and sigmoid probabilities only
 //   cachegrad scatter-add of the cached tables' gradient rows
 //   adagrad   tf.keras Adagrad over the flat fp32 parameter buffer + refresh of the bf16
 //             K-major weight copies (W and W^T) consumed by the wgmma GEMMs
@@ -448,6 +449,39 @@ __global__ void __launch_bounds__(256) exb_head_row_kernel(HeadArgs a) {
     }
 }
 
+struct PredictArgs {
+    const __nv_bfloat16* H; int Hp;               // last hidden activation [B, Hp]
+    const float* wout;                            // [Hp] (ones-column entry = output bias)
+    const float* base;                            // [B] linear + FM / CIN / cross terms
+    float* logits; float* probs;                  // [B], [B]
+    int B;
+};
+
+// predict head (evaluation): one warp per batch row, any Hp: z = base + H[b,:] . wout, sigmoid(z).
+// Writes logits and probs only -- no loss, dlogit, dZ or gradient.
+__global__ void __launch_bounds__(256) exb_predict_head_kernel(PredictArgs a) {
+    exb::pdl_trigger();
+    exb::pdl_wait();
+    const int lane = threadIdx.x & 31;
+    const int b = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (b >= a.B) return;
+    const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(a.H + (size_t)b * a.Hp);
+    const float2* w2 = reinterpret_cast<const float2*>(a.wout);
+    float z = 0.f;
+    for (int n = lane; n < a.Hp / 2; n += 32) {
+        const float2 hv = __bfloat1622float2(h2[n]);
+        const float2 wv = w2[n];
+        z += hv.x * wv.x + hv.y * wv.y;
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
+    if (lane == 0) {
+        z += a.base[b];
+        a.logits[b] = z;
+        a.probs[b] = 1.f / (1.f + expf(-z));
+    }
+}
+
 // Scatter-add the gradient rows of the cached (replicated) embedding tables.
 // CTA = (cached feature, 256 batch rows), warp = 32 rows. The 32 gradient rows go through a
 // per-warp shared-memory tile; rows with the SAME id are grouped with __match_any_sync, the first
@@ -878,6 +912,18 @@ int exb_head(const void* args, int B, uint64_t stream) {
     return 0;
 }
 int exb_head_args_size() { return (int)sizeof(HeadArgs); }
+int exb_predict_head(const void* args, uint64_t stream) {
+    const PredictArgs a = *reinterpret_cast<const PredictArgs*>(args);
+    if (a.Hp < 2 || a.Hp % 2 || ((uintptr_t)a.H & 3) || ((uintptr_t)a.wout & 7) || !a.base || !a.logits || !a.probs) {
+        g_dense_err = "predict_head: even Hp, 4-byte aligned H, 8-byte aligned w_out, base / logits / probs required";
+        return -1;
+    }
+    const int grid = a.B > 0 ? (a.B + 7) / 8 : 1;
+    cudaError_t e = exb::launch_pdl(exb_predict_head_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, a);
+    if (e != cudaSuccess) { g_dense_err = cudaGetErrorString(e); return -1; }
+    return 0;
+}
+int exb_predict_args_size() { return (int)sizeof(PredictArgs); }
 int exb_cachegrad(uint64_t G32, long long xs, int col0, int Dp, uint64_t ids, int ncols, uint64_t cache_col,
                   uint64_t cache_off, int nc, uint64_t g_cache_emb, int B, uint64_t dlogit, uint64_t g_cache_lin,
                   uint64_t cache_vocab, uint64_t stream) {

@@ -26,6 +26,9 @@ interaction backward, filter-gradient GEMM) and the fold of the CIN embedding gr
 DCN-v2 adds the cross network on the A0 layout (csrc/cuda/cross_kernels.cu + the wgmma GEMM), 1 + 5 L launches for
 L layers: L x (U_l GEMM, cross forward) before the head; after the dX GEMM, the top of the cross backward and
 L x (P_l GEMM, weight-gradient GEMM, cross backward), the last of which folds the embedding gradient into G32.
+
+Evaluation (``predict_forward``; ``FusedTrainer.predict`` / ``evaluate``) runs the forward half alone: stateless pull,
+prep, the forward GEMMs, the CIN / cross forward and the predict head (logits + probabilities, dense_kernels.cu).
 """
 import ctypes
 import os
@@ -56,6 +59,11 @@ class _HeadArgs(ctypes.Structure):
                 ("G32", c_void_p), ("xs", c_longlong), ("lin0", c_int), ("ns", c_int), ("ids", c_void_p),
                 ("ncols", c_int), ("cache_col", c_void_p), ("cache_off", c_void_p), ("nc", c_int),
                 ("g_cache_lin", c_void_p), ("B", c_int), ("grad_scale", c_float)]
+
+
+class _PredictArgs(ctypes.Structure):
+    _fields_ = [("H", c_void_p), ("Hp", c_int), ("wout", c_void_p), ("base", c_void_p), ("logits", c_void_p),
+                ("probs", c_void_p), ("B", c_int)]
 
 
 _OPT_MAX_MATS = 8          # csrc/cuda/dense_kernels.cu: EXB_OPT_MAX_MATS (DNN layers + CIN layers)
@@ -124,6 +132,9 @@ def _lib():
         lib.exb_head.argtypes = [c_void_p, c_int, u64]
         lib.exb_prep_args_size.restype = c_int
         lib.exb_head_args_size.restype = c_int
+        lib.exb_predict_head.restype = c_int
+        lib.exb_predict_head.argtypes = [c_void_p, u64]
+        assert lib.exb_predict_args_size() == ctypes.sizeof(_PredictArgs), "PredictArgs ABI mismatch"
         lib.exb_cachegrad.restype = c_int
         lib.exb_cachegrad.argtypes = [u64, c_longlong, c_int, c_int, u64, c_int, u64, u64, c_int, u64, c_int, u64, u64, u64,
                                       u64]
@@ -414,6 +425,10 @@ class FusedCTR:
         self.base = torch.zeros(B, dtype=f32, device=dev)
         self.dlogit = torch.zeros(B, dtype=f32, device=dev)
         self.loss = torch.zeros(1, dtype=f32, device=dev)
+        self.logits = torch.zeros(B, dtype=f32, device=dev)       # predict_forward's outputs
+        self.probs = torch.zeros(B, dtype=f32, device=dev)
+        self._predict_args = _PredictArgs(self.H[-1].data_ptr(), self.Hp[-1], self.view("wout").data_ptr(),
+                                          self.base.data_ptr(), self.logits.data_ptr(), self.probs.data_ptr(), B)
         offs_c, o = [], 0
         for f in self.cached:
             offs_c.append(o)
@@ -673,6 +688,61 @@ class FusedCTR:
             _ck(self.lib.exb_refresh_bf16(self.view("X%d" % l).data_ptr(), self.xWb[l].data_ptr(), self.xWTb[l].data_ptr(),
                                           self.K0p, self.K0p, self._st()), "refresh_bf16")
 
+    def _forward(self, ids, dense, st, loss, opt_step):
+        """prep, the forward GEMMs and the CIN / cross branches on the rows in X32: leaves H[-1] and base for a
+        head. ``loss`` / ``opt_step``: device addresses prep clears / advances, 0 for neither."""
+        B, L, tn = self.B, len(self.hidden), self.mn_major
+        pa = _PrepArgs(self.X32.data_ptr(), self.XS, self.A0.data_ptr(), 0 if tn else self.A0T.data_ptr(), ids.data_ptr(), self.nf,
+                       dense.data_ptr(), self.nd, self.view("cache_emb").data_ptr(), self.view("cache_lin").data_ptr(),
+                       self.cache_col.data_ptr(), self.cache_off.data_ptr(), self.nc, self.view("wd").data_ptr(),
+                       self.view("bias").data_ptr(), self.S.data_ptr(), self.base.data_ptr(), B, self.K0p, self.Dp,
+                       self.nf, self.ns, self.lin0, int(self.use_fm), loss, opt_step)
+        _ck(self.lib.exb_prep(ctypes.byref(pa), B, self.Dp, st), "prep")
+        self._mark("prep")
+        dims = [self.K0p] + self.Hp
+        src = self.A0
+        if self.chain_fwd:
+            self.fwd_chain.launch(st)
+        else:
+            for l in range(L):
+                G.gemm_nt(src, self.Wb[l], B, self.Hp[l], dims[l], self.H[l], mode=G.EPI_FWD, relu=True,
+                          ones_col=self.Hp[l] - 1, outT=self.HT[l] if (l < L - 1 and not tn) else None, stream=st)
+                src = self.H[l]
+        self._mark("fwd_gemm")
+        if self.cin:
+            self._cin_forward(st)
+            self._mark("cin_fwd")
+        if self.dcn:
+            self._cross_forward(st, dense)
+            self._mark("cross_fwd")
+
+    # ---- forward-only pass (evaluation; all launches on the current stream)
+    def predict_forward(self, ids, dense):
+        """Logits and sigmoid probabilities of a full batch into ``self.logits`` / ``self.probs`` (fp32 [B]):
+        stateless pull of the rows into X32, prep (the training loss and the optimizer step counter untouched), the
+        forward GEMMs, the CIN / cross branches, then the predict head. No parameter, optimizer state, gradient,
+        sparse plan or table row changes -- but X32 and the other activation buffers are overwritten, so rows that
+        a training step prefetched into X32 are gone (``FusedTrainer`` makes the next step pull again)."""
+        B = self.B
+        assert ids.shape == (B, self.nf) and ids.dtype == torch.int64 and ids.is_contiguous()
+        assert dense.shape == (B, self.nd) and dense.dtype == torch.float32 and dense.is_contiguous()
+        st = self._st()
+        self.group.pull(ids, out=self.X32)
+        self._mark("pull")
+        self._forward(ids, dense, st, 0, 0)
+        _ck(self.lib.exb_predict_head(ctypes.byref(self._predict_args), st), "predict_head")
+        self._mark("predict_head")
+        return self.logits
+
+    def kernels_per_eval(self, metric=False):
+        """launches of our own kernels in one ``predict_forward`` (+ 1 for the metric update of an evaluation)"""
+        L = len(self.hidden)
+        prep = 1 if (self.mn_major and 128 % self.Dp == 0) else 2
+        n = 1 + prep + (1 if self.chain_fwd else L) + 1                # pull prep GEMMs head
+        n += 2 + 2 * len(self.cin_layers) if self.cin else 0          # gather + pool, per layer outer + GEMM
+        n += 2 * self.cross_layers if self.dcn else 0                 # per layer GEMM + cross forward
+        return n + (1 if metric else 0)
+
     # ---- one training step (all launches on the current stream)
     def forward_backward(self, ids, dense, labels, update=True, next_ids=None, pulled=False):
         """One training step. ``next_ids``: ids of the NEXT batch (a device tensor that stays unchanged until that
@@ -698,30 +768,8 @@ class FusedCTR:
             g.pull(ids, out=self.X32)
         self._mark("pull")
         tn = self.mn_major
-        pa = _PrepArgs(self.X32.data_ptr(), self.XS, self.A0.data_ptr(), 0 if tn else self.A0T.data_ptr(), ids.data_ptr(), self.nf,
-                       dense.data_ptr(), self.nd, self.view("cache_emb").data_ptr(), self.view("cache_lin").data_ptr(),
-                       self.cache_col.data_ptr(), self.cache_off.data_ptr(), self.nc, self.view("wd").data_ptr(),
-                       self.view("bias").data_ptr(), self.S.data_ptr(), self.base.data_ptr(), B, self.K0p, self.Dp,
-                       self.nf, self.ns, self.lin0, int(self.use_fm), self.loss.data_ptr(),
-                       self.opt_step.data_ptr() if update else 0)
-        _ck(lib.exb_prep(ctypes.byref(pa), B, self.Dp, st), "prep")
-        self._mark("prep")
+        self._forward(ids, dense, st, self.loss.data_ptr(), self.opt_step.data_ptr() if update else 0)
         dims = [self.K0p] + self.Hp
-        src = self.A0
-        if self.chain_fwd:
-            self.fwd_chain.launch(st)
-        else:
-            for l in range(L):
-                G.gemm_nt(src, self.Wb[l], B, self.Hp[l], dims[l], self.H[l], mode=G.EPI_FWD, relu=True,
-                          ones_col=self.Hp[l] - 1, outT=self.HT[l] if (l < L - 1 and not tn) else None, stream=st)
-                src = self.H[l]
-        self._mark("fwd_gemm")
-        if self.cin:
-            self._cin_forward(st)
-            self._mark("cin_fwd")
-        if self.dcn:
-            self._cross_forward(st, dense)
-            self._mark("cross_fwd")
         row_head = tn and self.Hp[-1] <= 512       # merged row-wise head; cachegrad then owns the cached linear grads
         ha = _HeadArgs(self.H[-1].data_ptr(), self.Hp[-1], self.Hp[-1] - 1, self.view("wout").data_ptr(),
                        self.base.data_ptr(), labels.data_ptr(), self.dlogit.data_ptr(), self.loss.data_ptr(),
@@ -846,9 +894,10 @@ class FusedCTR:
         return n + (1 if self._ar is not None and not self._rider else 0)
 
     # ---- fp32 torch reference of the dense math on the current X32 (tests)
-    def reference(self, ids, dense, labels):
+    def reference(self, ids, dense, labels, return_logits=False):
         """returns (loss, grads dict) computed with torch autograd in fp32 from the same
-        parameters and the same pulled embeddings (self.X32 after a forward)."""
+        parameters and the same pulled embeddings (self.X32 after a forward); ``return_logits``: (loss, grads,
+        logits [B])."""
         B, nf, Dp, L = self.B, self.nf, self.Dp, len(self.hidden)
         theta = self.theta.detach().clone().requires_grad_(True)
         X = self.X32.detach().clone()
@@ -892,7 +941,10 @@ class FusedCTR:
             z = z + self._reference_cross(torch.cat([emb.view(B, nf, Dp)[:, :, :self.D].reshape(B, -1), dense], 1), theta)
         loss =torch.nn.functional.binary_cross_entropy_with_logits(z, labels)
         loss.backward()
-        return loss.detach(), {"theta": theta.grad, "emb": emb_leaf.grad, "lin": lin_leaf.grad}
+        grads = {"theta": theta.grad, "emb": emb_leaf.grad, "lin": lin_leaf.grad}
+        if return_logits:
+            return loss.detach(), grads, z.detach()
+        return loss.detach(), grads
 
     def _reference_cin(self, x, theta):
         """CIN(x) . w_cin for ``reference``: the eager zoo's ``models.ctr.CIN`` (plain torch) run on the filters in
@@ -957,7 +1009,11 @@ class FusedTrainer:
 
     Before the first capture every kernel of the step is launched eagerly twice through ``FusedCTR.warmup`` (lazy
     kernel loading and allocator growth may not happen inside a capture); the warm-up changes no parameter, so the
-    graph-driven trajectory is the eager one from the first step on."""
+    graph-driven trajectory is the eager one from the first step on.
+
+    ``predict(ids, dense)`` / ``evaluate(ids, dense, labels, metrics)``: the forward-only pass over n <= B rows,
+    replayed from one more graph (key ``"eval"``); an evaluation drops a prefetched next batch, whose step then
+    pulls up front."""
 
     supports_prefetch = True
     want_prefetch = True         # ``make_pipeline`` runs one batch ahead: the next batch's pull overlaps this step's tail
@@ -974,6 +1030,7 @@ class FusedTrainer:
         self._ar = model._ar
         self._x32_key = None         # key of the batch whose rows + plan the last step prefetched into X32
         self._warm = False
+        self._eval = None            # static eval inputs (ids, dense, labels, n on the device) of predict / evaluate
 
     def step(self, ids, dense, labels, next_ids=None, stable=False):
         """``stable=True``: the caller keeps the four input tensors alive at fixed addresses and refills them in place
@@ -1051,6 +1108,60 @@ class FusedTrainer:
             g._armed = saved            # capture only recorded launches: the device-side slots are untouched
         self._graphs[key] = gr
         return gr
+
+    # ---- evaluation: forward-only pass on the trainer's static, zero-padded eval buffers
+    def _eval_forward(self, ids, dense, labels=None):
+        """copy n <= B rows into the eval buffers (rows >= n zero), set n on the device, run the forward-only pass
+        (graph replay, or eagerly); returns n"""
+        m = self.m
+        n = ids.shape[0]
+        if not (1 <= n <= m.B) or ids.shape[1] != m.nf or dense.shape != (n, m.nd):
+            raise ValueError("evaluation takes 1 .. %d rows of ids [n, %d] and dense [n, %d]" % (m.B, m.nf, m.nd))
+        if labels is not None and labels.numel() != n:
+            raise ValueError("%d labels for %d rows" % (labels.numel(), n))
+        e = self._eval
+        if e is None:
+            dev = self.device
+            e = self._eval = {"ids": torch.zeros(m.B, m.nf, dtype=torch.int64, device=dev),
+                              "dense": torch.zeros(m.B, m.nd, dtype=torch.float32, device=dev),
+                              "labels": torch.zeros(m.B, dtype=torch.float32, device=dev),
+                              "n": torch.zeros(1, dtype=torch.int32, device=dev)}
+        for name, src in (("ids", ids), ("dense", dense), ("labels", labels)):
+            if src is None:
+                continue
+            e[name][:n].copy_(src.reshape(e[name][:n].shape), non_blocking=True)
+            e[name][n:].zero_()
+        e["n"].fill_(n)
+        # the forward overwrites X32: rows (and, v2, the plan) a step prefetched for the next batch are dropped the
+        # way ``step`` drops a prefetch that is not followed, and that step pulls up front again
+        if self._x32_key is not None:
+            if getattr(m.group, "v2", False):
+                m.group.reset_slot(0)
+            self._x32_key = None
+        if not self.use_graph:
+            m.predict_forward(e["ids"], e["dense"])
+            return n
+        gr = self._graphs.get("eval")
+        if gr is None:
+            torch.cuda.synchronize(self.device)
+            m.predict_forward(e["ids"], e["dense"])    # side-effect free: one eager run loads every kernel
+            torch.cuda.synchronize(self.device)
+            gr = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(gr):
+                m.predict_forward(e["ids"], e["dense"])
+            self._graphs["eval"] = gr
+        gr.replay()
+        return n
+
+    def predict(self, ids, dense):
+        """probabilities of n <= B rows (device ids [n, nf] int64, dense [n, nd] fp32) as a new fp32 tensor [n]"""
+        n = self._eval_forward(ids, dense)
+        return self.m.probs[:n].clone()
+
+    def evaluate(self, ids, dense, labels, metrics):
+        """forward-only pass over n <= B rows, accumulated into ``metrics`` (``models.metrics.BinaryMetrics``)"""
+        self._eval_forward(ids, dense, labels)
+        metrics.update(self.m.logits, self._eval["labels"], n=self._eval["n"])
 
     def make_pipeline(self, batch, num_sparse, num_dense):
         from .trainer import _Pipeline

@@ -222,58 +222,87 @@ __device__ __forceinline__ void mma_tile(float (&acc)[BN / 2], const uint8_t* sA
 template <int BN>
 __device__ __forceinline__ void epilogue_tile(const GemmEpi& E, float (&acc)[BN / 2], int m_blk, int n_blk, int g,
                                               uint8_t* stage, int qstride, const CUtensorMap* tO, const CUtensorMap* tT) {
+    // kept in registers: in the chain the descriptor lives in shared memory, and the staging stores below could
+    // alias it for the compiler, which then re-reads every field after every store
+    const int mode = E.mode, relu = E.relu, ones_col = E.ones_col, fm_cols = E.fm_cols, N = E.N, D = E.D;
+    const bool has_t = E.outT != nullptr;
     const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
-    const bool f32out = (E.mode == EPI_DW || E.mode == EPI_DX_FM);
+    const bool f32out = (mode == EPI_DW || mode == EPI_DX_FM);
     const int q = 2 * g + (w >> 1);
     uint8_t* wstage = stage + q * qstride;
     uint8_t* tstage = wstage + BN * 128;
+    // The global operands of the fused math (relu mask; FM embedding row and S) are read-only loads issued LOOK
+    // column pairs at a time, ahead of the math and staging stores of those pairs, so the loads of a group are in
+    // flight together rather than one memory round trip per pair. At two CTAs per SM a thread has 96 registers:
+    // BN = 64 fits four pairs (ptxas -v: 86 registers single launch, 96 chain, no spills; eight spill in the
+    // chain); BN = 128 with its 64 accumulators takes one pair at a time and spills 44 bytes.
+    constexpr int LOOK = BN == 64 ? 4 : 1;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
         const int qrow = (w & 1) * 16 + (l >> 2) + 8 * i;
         const int row = m_blk * BM + q * 32 + qrow;
         const bool rv = row < E.M;
         // dlogit / S / emb exist only when the tile has FM columns (fm_cols = 0: plain fp32 dX, null pointers)
-        const float dl = (E.mode == EPI_DX_FM && rv && n_blk * BN < E.fm_cols) ? E.dlogit[row] : 0.f;
+        const bool fm_row = mode == EPI_DX_FM && rv && n_blk * BN < fm_cols;
+        const float dl = fm_row ? __ldg(E.dlogit + row) : 0.f;
+        const __nv_bfloat16* mrow = E.mask + (size_t)row * E.ldmask;
+        const float* erow = E.emb + (size_t)row * E.ldemb;
+        const float* sb = E.S + (size_t)row * D;
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-            const int c = 8 * j + 2 * (l & 3);
-            const int n = n_blk * BN + c;
-            float x[2] = {acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]};
-            if (E.mode == EPI_FWD) {
+        for (int j0 = 0; j0 < BN / 8; j0 += LOOK) {
+            float4 v[LOOK];     // relu mask (x, y) | FM embedding pair (x, y) and S at its two columns (z, w)
 #pragma unroll
-                for (int u = 0; u < 2; ++u) {
-                    if (E.relu) x[u] = fmaxf(x[u], 0.f);
-                    if (n + u == E.ones_col) x[u] = 1.f;
-                    if (n + u >= E.N) x[u] = 0.f;
+            for (int jj = 0; jj < LOOK; ++jj) {
+                const int n = n_blk * BN + 8 * (j0 + jj) + 2 * (l & 3);
+                v[jj] = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (mode == EPI_DX) {
+                    if (rv && n < N) {
+                        const float2 mk = __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(mrow + n)));
+                        v[jj].x = mk.x; v[jj].y = mk.y;
+                    }
+                } else if (fm_row && n < fm_cols) {
+                    // per column pair: n is even and fm_cols = nf * Dp a multiple of 4, so n + 1 < fm_cols as well.
+                    // fm_cols need not be a multiple of 32 (nf * Dp = 208 at dim 8): the columns of a partial
+                    // 32-column group are embedding columns too and need the FM term
+                    const float2 e2 = __ldg(reinterpret_cast<const float2*>(erow + n));
+                    v[jj] = make_float4(e2.x, e2.y, __ldg(sb + n % D), __ldg(sb + (n + 1) % D));
                 }
-            } else if (E.mode == EPI_DX) {
-                float2 mk = make_float2(0.f, 0.f);
-                if (rv && n < E.N) mk = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(E.mask + (size_t)row * E.ldmask + n));
-                const float mv[2] = {mk.x, mk.y};
-#pragma unroll
-                for (int u = 0; u < 2; ++u)
-                    if (!rv || !(mv[u] > 0.f) || n + u == E.ones_col || n + u >= E.N) x[u] = 0.f;
-            } else if (E.mode == EPI_DX_FM && rv && n < E.fm_cols) {
-                // per column pair: n is even and fm_cols = nf * Dp a multiple of 4, so n + 1 < fm_cols as well.
-                // fm_cols need not be a multiple of 32 (nf * Dp = 208 at dim 8): the columns of a partial
-                // 32-column group are embedding columns too and need the FM term
-                const float2 e2 = *reinterpret_cast<const float2*>(E.emb + (size_t)row * E.ldemb + n);
-                const float* sb = E.S + (size_t)row * E.D;
-                x[0] += dl * (sb[n % E.D] - e2.x);
-                x[1] += dl * (sb[(n + 1) % E.D] - e2.y);
             }
-            // registers -> swizzled staging tile (rows of 128 bytes, 16-byte chunk index ^ (row & 7))
-            if (f32out) {   // [32 rows][32 fp32] per 32 columns
-                const int cc = c & 31;
-                *reinterpret_cast<float2*>(wstage + (c >> 5) * 4096 + qrow * 128 + ((((cc >> 2) ^ (qrow & 7))) << 4) + (cc & 3) * 4) =
-                    make_float2(x[0], x[1]);
-            } else {        // [32 rows][64 bf16] per 64 columns
-                const int cc = c & 63;
-                *reinterpret_cast<__nv_bfloat162*>(wstage + (c >> 6) * 4096 + qrow * 128 + ((((cc >> 3) ^ (qrow & 7))) << 4) + (cc & 7) * 2) =
-                    __floats2bfloat162_rn(x[0], x[1]);
-                if (E.outT) {   // [BN n][32 rows] bf16
-                    *reinterpret_cast<__nv_bfloat16*>(tstage + c * 64 + qrow * 2) = __float2bfloat16_rn(x[0]);
-                    *reinterpret_cast<__nv_bfloat16*>(tstage + (c + 1) * 64 + qrow * 2) = __float2bfloat16_rn(x[1]);
+#pragma unroll
+            for (int jj = 0; jj < LOOK; ++jj) {
+                const int j = j0 + jj;
+                const int c = 8 * j + 2 * (l & 3);
+                const int n = n_blk * BN + c;
+                float x[2] = {acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]};
+                if (mode == EPI_FWD) {
+#pragma unroll
+                    for (int u = 0; u < 2; ++u) {
+                        if (relu) x[u] = fmaxf(x[u], 0.f);
+                        if (n + u == ones_col) x[u] = 1.f;
+                        if (n + u >= N) x[u] = 0.f;
+                    }
+                } else if (mode == EPI_DX) {
+                    const float mv[2] = {v[jj].x, v[jj].y};
+#pragma unroll
+                    for (int u = 0; u < 2; ++u)
+                        if (!rv || !(mv[u] > 0.f) || n + u == ones_col || n + u >= N) x[u] = 0.f;
+                } else if (fm_row && n < fm_cols) {
+                    x[0] += dl * (v[jj].z - v[jj].x);
+                    x[1] += dl * (v[jj].w - v[jj].y);
+                }
+                // registers -> swizzled staging tile (rows of 128 bytes, 16-byte chunk index ^ (row & 7))
+                if (f32out) {   // [32 rows][32 fp32] per 32 columns
+                    const int cc = c & 31;
+                    *reinterpret_cast<float2*>(wstage + (c >> 5) * 4096 + qrow * 128 + ((((cc >> 2) ^ (qrow & 7))) << 4) + (cc & 3) * 4) =
+                        make_float2(x[0], x[1]);
+                } else {        // [32 rows][64 bf16] per 64 columns
+                    const int cc = c & 63;
+                    *reinterpret_cast<__nv_bfloat162*>(wstage + (c >> 6) * 4096 + qrow * 128 + ((((cc >> 3) ^ (qrow & 7))) << 4) + (cc & 7) * 2) =
+                        __floats2bfloat162_rn(x[0], x[1]);
+                    if (has_t) {    // [BN n][32 rows] bf16
+                        *reinterpret_cast<__nv_bfloat16*>(tstage + c * 64 + qrow * 2) = __float2bfloat16_rn(x[0]);
+                        *reinterpret_cast<__nv_bfloat16*>(tstage + (c + 1) * 64 + qrow * 2) = __float2bfloat16_rn(x[1]);
+                    }
                 }
             }
         }
@@ -628,7 +657,11 @@ int pick_bn(int M, int N, int K) {
     // default 64: the step's GEMMs (M = batch, N <= 1 728) have few tiles, and 64-wide tiles give twice as many to
     // spread over the SMs. Tall, short-K products (the CIN input-gradient GEMM: M 36 864, N 1 728, K 128 -- two
     // k-blocks per tile, thousands of tiles) take 128: their tiles are mostly set-up and epilogue, and the wider
-    // tile halves their number. The two widths have not been timed against each other on H100.
+    // tile halves their number. The DeepFM step keeps 64 by measurement on H100 (docs/benchmark.md): with 128 for
+    // the two 448-K forward GEMMs only (fwd2, fwd3), bench.py ran 0.361-0.362 ms/step against 0.332 at 64, three
+    // runs each, alternated; 128 for all three forward GEMMs was slower as well. Isolated back-to-back launches of
+    // one GEMM (benchmarks/step_gemms.py) do not predict this: they swing by more than the width difference
+    // between runs of the same code.
     if (K <= 128 && N >= 512 && M >= 8192) return 128;
     return 64;
 }

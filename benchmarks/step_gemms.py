@@ -6,7 +6,8 @@
 For every GEMM of the step (fwd1..3, then dX3, dW3, dX2, dW2, dX1 with the FM term, dW1 split-K) this prints, per
 single-launch tile width BN: the time of the single launch (``gemm_nt`` / ``gemm_tn``), the achieved TFLOP/s and the
 operand bytes the tiles read from L2, and the time of the same GEMM as a one-GEMM persistent chain (64-wide tiles).
-It also times the whole forward (three single launches, and the forward chain) and the whole backward (six single
+A last row, "dX1 (no FM)", is dX1 with a plain fp32 store (``fm_cols=0``): the same GEMM without the FM epilogue's
+operands, so its gap to "dX1 (FM)" bounds what the FM epilogue costs. It also times the whole forward (three single launches, and the forward chain) and the whole backward (six single
 launches, and the backward chain that the step runs). Device-timed with CUDA events over
 ``--steps`` launches after ``--warmup``; the card and its power limit are read in the same run.
 
@@ -83,6 +84,9 @@ def child(bn):
 
     # (name, M, N, K, single launch, chain descriptor) -- the step's GEMMs as FusedCTR issues them
     gemms = []
+    # dX1 with a plain fp32 store and no FM operands (fm_cols = 0): timed after the step's GEMMs, not part of the
+    # whole forward / backward. Its gap to "dX1 (FM)" is what the FM epilogue costs.
+    nofm = []
     src = m.A0
     for l in range(L):
         def fwd(l=l, src=src):
@@ -107,6 +111,9 @@ def child(bn):
                 G.gemm_nt(m.dZ[0], m.WTb[0], B, m.K0p, Hp[0], m.G32, mode=G.EPI_DX_FM, stream=st, **fm)
             gemms.append(("dX1 (FM)", B, m.K0p, Hp[0], dx,
                           lambda fm=fm: G.chain_nt(m.dZ[0], m.WTb[0], B, m.K0p, Hp[0], m.G32, mode=G.EPI_DX_FM, **fm)))
+            nofm.append(("dX1 (no FM)", B, m.K0p, Hp[0],
+                         lambda: G.gemm_nt(m.dZ[0], m.WTb[0], B, m.K0p, Hp[0], m.G32, mode=G.EPI_DX_FM, fm_cols=0, stream=st),
+                         lambda: G.chain_nt(m.dZ[0], m.WTb[0], B, m.K0p, Hp[0], m.G32, mode=G.EPI_DX_FM, fm_cols=0)))
         prev = m.A0 if l == 0 else m.H[l - 1]
 
         def dw(l=l, prev=prev, gW=gW):
@@ -136,7 +143,7 @@ def child(bn):
 
     name, power = card()
     out = []
-    for nm, M, N, K, single, desc in gemms:
+    for nm, M, N, K, single, desc in gemms + nofm:
         row = {"gemm": nm, "M": M, "N": N, "K": K, "bn": bn, "single_us": timed(single)}
         row["chain_us"] = run_chain([desc()])
         row["gflop"] = 2.0 * M * N * K / 1e9

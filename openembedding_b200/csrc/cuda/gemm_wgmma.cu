@@ -16,6 +16,8 @@
 //   EPI_DX    relu mask from the forward activation, bf16 store (+ transposed copy)
 //   EPI_DW    split-K partial sums, fp32 TMA reduce-add
 //   EPI_DX_FM fp32 store of the embedding gradient with the FM second-order term fused
+// The relu mask and the FM embedding columns reach the epilogue as a TMA-loaded source tile in the staging tile
+// (epi_src_boxes / load_epi_src).
 //
 // Every GEMM of the training step (3 forward, 3 dX, 3 dW) is this one kernel. Operands reach wgmma
 // either K-major (transposed copies written by the producing epilogue) or MN-major (the dW products
@@ -215,9 +217,39 @@ __device__ __forceinline__ void mma_tile(float (&acc)[BN / 2], const uint8_t* sA
     if (nkb > 0) release(kiter + nkb - 1);
 }
 
+// Epilogue source tile: the operand the fused math reads elementwise beside the accumulator -- the relu mask of
+// EPI_DX (bf16 [M, N], 64-column boxes) or the FM embedding columns of EPI_DX_FM (fp32 [M, fm_cols], 32-column
+// boxes). A box of it is laid out exactly like the output staging tile it lands in (rows of 128 bytes, 128B
+// swizzle), so the epilogue reads each element from the address it then writes its result to.
+// Boxes per 32-row quarter of a 128 x BN tile; 0: the tile has no source (every other epilogue, fm_cols = 0, a
+// tile right of the embedding columns).
+template <int BN>
+__device__ __forceinline__ int epi_src_boxes(int mode, int fm_cols, int N, int n_blk) {
+    const int n0 = n_blk * BN;
+    if (mode == EPI_DX) return min(BN / 64, (N - n0 + 63) / 64);
+    if (mode == EPI_DX_FM && fm_cols > n0) return min(BN / 32, (fm_cols - n0 + 31) / 32);
+    return 0;
+}
+// TMA loads of warpgroup g's two staging quarters, completing on `bar` (issued by one thread). Quarters that start
+// at or past row M are skipped: their rows are masked in the epilogue. Rows >= M of a partial quarter and columns
+// past the tensor's width arrive zero-filled.
+template <int BN>
+__device__ __forceinline__ void load_epi_src(const CUtensorMap* tE, uint64_t* bar, uint8_t* stage, int qstride, int g,
+                                             int m_blk, int n_blk, int boxes, int M, bool f32) {
+    const int row0 = m_blk * BM + 2 * g * 32;
+    const int quarters = row0 >= M ? 0 : (row0 + 32 >= M ? 1 : 2);
+    mbar_expect_tx(bar, (uint32_t)(quarters * boxes * 4096));
+#pragma unroll 1
+    for (int qq = 0; qq < quarters; ++qq)
+#pragma unroll 1
+        for (int h = 0; h < boxes; ++h)
+            tma_load_2d(stage + (2 * g + qq) * qstride + h * 4096, tE, bar, n_blk * BN + (f32 ? 32 : 64) * h, row0 + 32 * qq);
+}
+
 // Fused epilogue of warpgroup g: accumulator fragment -> fused math -> 128B-swizzled staging tiles (one per
 // 32-row quarter of the tile, `qstride` bytes apart; out tiles first, the outT tile at +BN*128) -> TMA stores
 // issued by the warpgroup's first thread (committed as one bulk group; the caller waits on it).
+// EPI_DX / EPI_DX_FM: the caller has landed the epilogue source tile in the staging tiles (load_epi_src).
 // wgmma m64nN fragment: thread (warp w, lane l) holds rows 16 w + l/4 (+8) and columns 8 j + 2 (l%4) (+1).
 template <int BN>
 __device__ __forceinline__ void epilogue_tile(const GemmEpi& E, float (&acc)[BN / 2], int m_blk, int n_blk, int g,
@@ -231,12 +263,10 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpi& E, float (&acc)[BN 
     const int q = 2 * g + (w >> 1);
     uint8_t* wstage = stage + q * qstride;
     uint8_t* tstage = wstage + BN * 128;
-    // The global operands of the fused math (relu mask; FM embedding row and S) are read-only loads issued LOOK
-    // column pairs at a time, ahead of the math and staging stores of those pairs, so the loads of a group are in
-    // flight together rather than one memory round trip per pair. At two CTAs per SM a thread has 96 registers:
-    // BN = 64 fits four pairs (ptxas -v: 86 registers single launch, 96 chain, no spills; eight spill in the
-    // chain); BN = 128 with its 64 accumulators takes one pair at a time and spills 44 bytes.
-    constexpr int LOOK = BN == 64 ? 4 : 1;
+    // The one global operand left is S of the FM term ([M, D] fp32, small and L2-resident): read-only loads of SG
+    // column pairs issued together, ahead of the math and staging stores of those pairs. At two CTAs per SM a
+    // thread has 96 registers; BN = 128 with its 64 accumulators takes fewer pairs at a time.
+    constexpr int SG = BN == 64 ? BN / 8 : 2;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
         const int qrow = (w & 1) * 16 + (l >> 2) + 8 * i;
@@ -245,35 +275,31 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpi& E, float (&acc)[BN 
         // dlogit / S / emb exist only when the tile has FM columns (fm_cols = 0: plain fp32 dX, null pointers)
         const bool fm_row = mode == EPI_DX_FM && rv && n_blk * BN < fm_cols;
         const float dl = fm_row ? __ldg(E.dlogit + row) : 0.f;
-        const __nv_bfloat16* mrow = E.mask + (size_t)row * E.ldmask;
-        const float* erow = E.emb + (size_t)row * E.ldemb;
         const float* sb = E.S + (size_t)row * D;
 #pragma unroll
-        for (int j0 = 0; j0 < BN / 8; j0 += LOOK) {
-            float4 v[LOOK];     // relu mask (x, y) | FM embedding pair (x, y) and S at its two columns (z, w)
+        for (int j0 = 0; j0 < BN / 8; j0 += SG) {
+            float2 s[SG];       // S at the two columns of the pair (the FM term's dimension n % D)
 #pragma unroll
-            for (int jj = 0; jj < LOOK; ++jj) {
+            for (int jj = 0; jj < SG; ++jj) {
                 const int n = n_blk * BN + 8 * (j0 + jj) + 2 * (l & 3);
-                v[jj] = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (mode == EPI_DX) {
-                    if (rv && n < N) {
-                        const float2 mk = __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(mrow + n)));
-                        v[jj].x = mk.x; v[jj].y = mk.y;
-                    }
-                } else if (fm_row && n < fm_cols) {
-                    // per column pair: n is even and fm_cols = nf * Dp a multiple of 4, so n + 1 < fm_cols as well.
-                    // fm_cols need not be a multiple of 32 (nf * Dp = 208 at dim 8): the columns of a partial
-                    // 32-column group are embedding columns too and need the FM term
-                    const float2 e2 = __ldg(reinterpret_cast<const float2*>(erow + n));
-                    v[jj] = make_float4(e2.x, e2.y, __ldg(sb + n % D), __ldg(sb + (n + 1) % D));
-                }
+                s[jj] = make_float2(0.f, 0.f);
+                // per column pair: n is even and fm_cols = nf * Dp a multiple of 4, so n + 1 < fm_cols as well.
+                // fm_cols need not be a multiple of 32 (nf * Dp = 208 at dim 8): the columns of a partial
+                // 32-column group are embedding columns too and need the FM term
+                if (fm_row && n < fm_cols) s[jj] = make_float2(__ldg(sb + n % D), __ldg(sb + (n + 1) % D));
             }
 #pragma unroll
-            for (int jj = 0; jj < LOOK; ++jj) {
+            for (int jj = 0; jj < SG; ++jj) {
                 const int j = j0 + jj;
                 const int c = 8 * j + 2 * (l & 3);
                 const int n = n_blk * BN + c;
                 float x[2] = {acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]};
+                // this pair's slot in the swizzled staging tile (rows of 128 bytes, 16-byte chunk index ^ (row & 7)):
+                // fp32 [32 rows][32 fp32] per 32 columns | bf16 [32 rows][64 bf16] per 64 columns
+                const int cc = f32out ? (c & 31) : (c & 63);
+                uint8_t* slot = f32out
+                    ? wstage + (c >> 5) * 4096 + qrow * 128 + ((((cc >> 2) ^ (qrow & 7))) << 4) + (cc & 3) * 4
+                    : wstage + (c >> 6) * 4096 + qrow * 128 + ((((cc >> 3) ^ (qrow & 7))) << 4) + (cc & 7) * 2;
                 if (mode == EPI_FWD) {
 #pragma unroll
                     for (int u = 0; u < 2; ++u) {
@@ -282,23 +308,21 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpi& E, float (&acc)[BN 
                         if (n + u >= N) x[u] = 0.f;
                     }
                 } else if (mode == EPI_DX) {
-                    const float mv[2] = {v[jj].x, v[jj].y};
+                    float2 mk = make_float2(0.f, 0.f);     // relu mask, from the source tile
+                    if (rv && n < N) mk = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(slot));
+                    const float mv[2] = {mk.x, mk.y};
 #pragma unroll
                     for (int u = 0; u < 2; ++u)
                         if (!rv || !(mv[u] > 0.f) || n + u == ones_col || n + u >= N) x[u] = 0.f;
                 } else if (fm_row && n < fm_cols) {
-                    x[0] += dl * (v[jj].z - v[jj].x);
-                    x[1] += dl * (v[jj].w - v[jj].y);
+                    const float2 e = *reinterpret_cast<const float2*>(slot);   // embedding pair, from the source tile
+                    x[0] += dl * (s[jj].x - e.x);
+                    x[1] += dl * (s[jj].y - e.y);
                 }
-                // registers -> swizzled staging tile (rows of 128 bytes, 16-byte chunk index ^ (row & 7))
-                if (f32out) {   // [32 rows][32 fp32] per 32 columns
-                    const int cc = c & 31;
-                    *reinterpret_cast<float2*>(wstage + (c >> 5) * 4096 + qrow * 128 + ((((cc >> 2) ^ (qrow & 7))) << 4) + (cc & 3) * 4) =
-                        make_float2(x[0], x[1]);
-                } else {        // [32 rows][64 bf16] per 64 columns
-                    const int cc = c & 63;
-                    *reinterpret_cast<__nv_bfloat162*>(wstage + (c >> 6) * 4096 + qrow * 128 + ((((cc >> 3) ^ (qrow & 7))) << 4) + (cc & 7) * 2) =
-                        __floats2bfloat162_rn(x[0], x[1]);
+                if (f32out) {
+                    *reinterpret_cast<float2*>(slot) = make_float2(x[0], x[1]);
+                } else {
+                    *reinterpret_cast<__nv_bfloat162*>(slot) = __floats2bfloat162_rn(x[0], x[1]);
                     if (has_t) {    // [BN n][32 rows] bf16
                         *reinterpret_cast<__nv_bfloat16*>(tstage + c * 64 + qrow * 2) = __float2bfloat16_rn(x[0]);
                         *reinterpret_cast<__nv_bfloat16*>(tstage + (c + 1) * 64 + qrow * 2) = __float2bfloat16_rn(x[1]);
@@ -345,7 +369,7 @@ template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 2)
 exb_gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmT,
-                      GemmEpi E, int num_k_blocks, int k_blocks_per_split) {
+                      const __grid_constant__ CUtensorMap tmE, GemmEpi E, int num_k_blocks, int k_blocks_per_split) {
     static_assert(BN == 64 || BN == 128, "tile width");
     constexpr int STAGES = stages_for<BN>();
     constexpr int B_BYTES = BN * BK * 2;
@@ -358,6 +382,7 @@ exb_gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     uint8_t* sB = smem + STAGES * A_BYTES;
     uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_BYTES);
     uint64_t* empty = full + STAGES;
+    uint64_t* srcfull = empty + STAGES;            // per warpgroup: its quarters of the epilogue source tile landed
 
     exb::pdl_trigger();   // the next kernel of the step may be scheduled once all CTAs are resident
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -380,6 +405,7 @@ exb_gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], (uint32_t)(NUM_CONSUMER_WARPS * C)); }
+        mbar_init(&srcfull[0], 1); mbar_init(&srcfull[1], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
@@ -428,6 +454,13 @@ exb_gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         if (threadIdx.x == 0) GSTAMP(3);
         // the staging tiles alias the stage ring: both warpgroups' wgmma reads must have retired
         named_bar_sync(1, 32 * NUM_CONSUMER_WARPS);
+        // so the epilogue source tile can only be requested now: one bulk round trip per warpgroup
+        const int boxes = epi_src_boxes<BN>(E.mode, E.fm_cols, E.N, n_blk);
+        if (boxes) {
+            if ((threadIdx.x & 127) == 0)
+                load_epi_src<BN>(&tmE, &srcfull[g], smem, QSTAGE, g, m_blk, n_blk, boxes, E.M, E.mode == EPI_DX_FM);
+            mbar_wait(&srcfull[g], 0);
+        }
         epilogue_tile<BN>(E, acc, m_blk, n_blk, g, smem, QSTAGE, &tmO, &tmT);
         if ((threadIdx.x & 127) == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
         if (threadIdx.x == 0) GSTAMP(4);
@@ -461,8 +494,8 @@ constexpr int CH_B_BYTES = CH_BN * BK * 2;
 constexpr int CH_MAX_PROB = 8;
 constexpr int CH_MAX_MB = 64;                 // row blocks per problem tracked by the ready counters
 
-struct ChainMaps { CUtensorMap tmA, tmB, tmO; };
-struct ChainMapsAll { ChainMaps m[CH_MAX_PROB]; };    // passed as a __grid_constant__ parameter (3 KB): descriptors in param space
+struct ChainMaps { CUtensorMap tmA, tmB, tmO, tmE; };  // tmE: epilogue source tile (zeroed when the GEMM has none)
+struct ChainMapsAll { ChainMaps m[CH_MAX_PROB]; };    // passed as a __grid_constant__ parameter (4 KB): descriptors in param space
 struct ChainMeta {
     GemmEpi E;
     int m_tiles, n_tiles, splits, nkb, per;
@@ -500,7 +533,11 @@ exb_gemm_chain_kernel(const __grid_constant__ ChainMapsAll MAPS, const ChainMeta
     uint8_t* sStage = sB + CH_STAGES * CH_B_BYTES;                 // 4 quarters x 8 KB (1024-byte aligned)
     uint64_t* full = reinterpret_cast<uint64_t*>(sStage + 4 * 8192);
     uint64_t* empty = full + CH_STAGES;
-    ChainMeta* M = reinterpret_cast<ChainMeta*>(empty + CH_STAGES);
+    // per consumer warpgroup g, for its two staging quarters: sfree -- the TMA store of its previous tile has read
+    // them; srcfull -- the epilogue source boxes of its current tile landed in them
+    uint64_t* sfree = empty + CH_STAGES;
+    uint64_t* srcfull = sfree + 2;
+    ChainMeta* M = reinterpret_cast<ChainMeta*>(srcfull + 2);
 
     exb::pdl_trigger();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -508,6 +545,7 @@ exb_gemm_chain_kernel(const __grid_constant__ ChainMapsAll MAPS, const ChainMeta
         reinterpret_cast<uint32_t*>(M)[i] = reinterpret_cast<const uint32_t*>(metas)[i];     // host-written
     if (threadIdx.x == 0) {
         for (int i = 0; i < CH_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], NUM_CONSUMER_WARPS); }
+        for (int i = 0; i < 2; ++i) { mbar_init(&sfree[i], 1); mbar_init(&srcfull[i], 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -515,8 +553,8 @@ exb_gemm_chain_kernel(const __grid_constant__ ChainMapsAll MAPS, const ChainMeta
 
     if (warp == PRODUCER_WARP) {
         if (lane == 0) {   // ===== TMA producer
-            uint32_t kiter = 0;
-            for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+            uint32_t kiter = 0, tile = 0;
+            for (int item = blockIdx.x; item < total_items; item += gridDim.x, ++tile) {
                 int p, m_blk, n_blk, z;
                 ch_decode(M, nprob, item, p, m_blk, n_blk, z);
                 const ChainMeta& Q = M[p];
@@ -536,7 +574,21 @@ exb_gemm_chain_kernel(const __grid_constant__ ChainMapsAll MAPS, const ChainMeta
                 }
                 const CUtensorMap* tA = &maps[p].tmA;
                 const CUtensorMap* tB = &maps[p].tmB;
+                const int boxes = epi_src_boxes<CH_BN>(Q.E.mode, Q.E.fm_cols, Q.E.N, n_blk);
+                // Staging hand-off, after the ring stages that are free while the consumers finish the previous
+                // tile and before the last k-block: wait until both warpgroups' stores of the previous tile have read
+                // the staging quarters, then load this tile's epilogue source into them. Waiting first would
+                // serialise the ring behind the store; waiting before the last k-block keeps a consumer from
+                // completing this tile's hand-off before the wait for the previous one (one phase in flight).
+                const int handoff = kb0 + min(CH_STAGES, kb1 - kb0 - 1);
                 for (int kb = kb0; kb < kb1; ++kb, ++kiter) {
+                    if (kb == handoff) {
+                        if (tile > 0) { mbar_wait(&sfree[0], (tile - 1) & 1u); mbar_wait(&sfree[1], (tile - 1) & 1u); }
+                        if (boxes)
+                            for (int g = 0; g < 2; ++g)
+                                load_epi_src<CH_BN>(&maps[p].tmE, &srcfull[g], sStage, 8192, g, m_blk, n_blk, boxes, Q.E.M,
+                                                    Q.E.mode == EPI_DX_FM);
+                    }
                     const int s = kiter % CH_STAGES;
                     const uint32_t ph = (kiter / CH_STAGES) & 1u;
                     mbar_wait(&empty[s], ph ^ 1u);
@@ -555,7 +607,7 @@ exb_gemm_chain_kernel(const __grid_constant__ ChainMapsAll MAPS, const ChainMeta
     } else {
         // ===== consumer warpgroups: main loop + epilogue of every item of this CTA
         const int g = warp >> 2;
-        uint32_t kiter = 0;
+        uint32_t kiter = 0, nsrc = 0;
         float acc[CH_BN / 2];
         for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
             int p, m_blk, n_blk, z;
@@ -568,6 +620,7 @@ exb_gemm_chain_kernel(const __grid_constant__ ChainMapsAll MAPS, const ChainMeta
             const int mn = __shfl_sync(0xffffffffu, Q.E.mn_major, 0);
             mma_tile<CH_BN>(acc, sA, sB, full, empty, CH_STAGES, kiter, nk, mn != 0, g, 1);
             kiter += nk;
+            if (epi_src_boxes<CH_BN>(Q.E.mode, Q.E.fm_cols, Q.E.N, n_blk)) mbar_wait(&srcfull[g], (nsrc++) & 1u);
             epilogue_tile<CH_BN>(Q.E, acc, m_blk, n_blk, g, sStage, 8192, &maps[p].tmO, &maps[p].tmO);
             if ((threadIdx.x & 127) == 0) {
                 if (Q.signal) {
@@ -581,6 +634,7 @@ exb_gemm_chain_kernel(const __grid_constant__ ChainMapsAll MAPS, const ChainMeta
                     // again; kernel completion makes the writes visible to the next kernel
                     asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
                 }
+                mbar_arrive(&sfree[g]);   // the producer may load the next tile's epilogue source into the staging
             }
             named_bar_sync(2 + g, 128);   // the staging tiles are free for the next item
         }
@@ -642,7 +696,27 @@ bool make_map_ex(CUtensorMap* map, CUtensorMapDataType dt, int esize, const void
 }
 
 template <int BN>
-constexpr size_t gemm_smem() { return stages_for<BN>() * (A_BYTES + BN * BK * 2) + (2 * stages_for<BN>() + 1) * 8 + 16 + 1024; }
+constexpr size_t gemm_smem() { return stages_for<BN>() * (A_BYTES + BN * BK * 2) + (2 * stages_for<BN>() + 2) * 8 + 16 + 1024; }
+
+// Tensor map of the epilogue source tile (epi_src_boxes): the relu mask of EPI_DX, the embedding columns of
+// EPI_DX_FM with fm_cols > 0. Returns true and leaves `map` untouched when the epilogue has no source.
+bool make_epi_src_map(CUtensorMap* map, int mode, int fm_cols, int M, int N, const void* mask, long long ldmask,
+                      const void* emb, long long ldemb) {
+    const bool dx = mode == EPI_DX, fm = mode == EPI_DX_FM && fm_cols > 0;
+    if (!dx && !fm) return true;
+    const void* p = dx ? mask : emb;
+    const long long ld = dx ? ldmask : ldemb;
+    const int esize = dx ? 2 : 4;
+    if (!p) { g_gemm_err = dx ? "gemm: EPI_DX needs the relu mask" : "gemm: fm_cols > 0 needs the embedding rows"; return false; }
+    // TMA: 16-byte aligned base and row stride
+    if (((uintptr_t)p & 15) != 0 || (ld * esize) % 16 != 0) {
+        g_gemm_err = dx ? "gemm: relu mask base / row stride not 16-byte aligned"
+                        : "gemm: embedding rows base / row stride not 16-byte aligned";
+        return false;
+    }
+    if (dx) return make_map_ex(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, p, M, N, ld, 64, 32, CU_TENSOR_MAP_SWIZZLE_128B);
+    return make_map_ex(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, p, M, fm_cols, ld, 32, 32, CU_TENSOR_MAP_SWIZZLE_128B);
+}
 
 // tile width: env EXB_GEMM_BN (64 | 128) overrides
 int pick_swap() {
@@ -668,7 +742,7 @@ int pick_bn(int M, int N, int K) {
 
 template <int BN>
 cudaError_t launch_gemm(dim3 grid, cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO,
-                        const CUtensorMap& tmT, const GemmEpi& E, int nkb, int per) {
+                        const CUtensorMap& tmT, const CUtensorMap& tmE, const GemmEpi& E, int nkb, int per) {
     static bool attr_set = false;
     if (!attr_set) {
         cudaFuncSetAttribute(exb_gemm_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem<BN>());
@@ -683,10 +757,10 @@ cudaError_t launch_gemm(dim3 grid, cudaStream_t stream, const CUtensorMap& tmA, 
         attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         attr[1].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = attr; cfg.numAttrs = exb::pdl_enabled() ? 2 : 1;
-        return cudaLaunchKernelEx(&cfg, exb_gemm_wgmma_kernel<BN>, tmA, tmB, tmO, tmT, E, nkb, per);
+        return cudaLaunchKernelEx(&cfg, exb_gemm_wgmma_kernel<BN>, tmA, tmB, tmO, tmT, tmE, E, nkb, per);
     }
     return exb::launch_pdl(exb_gemm_wgmma_kernel<BN>, grid, dim3(NUM_THREADS), gemm_smem<BN>(), stream, tmA, tmB, tmO, tmT,
-                           E, nkb, per);
+                           tmE, E, nkb, per);
 }
 
 // cluster size for the A-tile multicast: the largest divisor (<= EXB_GEMM_MC, <= 8) of the number of N tiles.
@@ -736,6 +810,8 @@ int exb_gemm_bf16_nt(uint64_t A, long long lda, uint64_t B, long long ldb, int M
         if (!make_map_ex(&tmO, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (const void*)out, M, (N + 63) / 64 * 64, ldo, 64, 32, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
     }
     tmT = tmO;
+    CUtensorMap tmE = tmO;    // placeholder when the epilogue has no source tile
+    if (!make_epi_src_map(&tmE, mode, fm_cols, M, N, (const void*)mask, ldmask, (const void*)emb, ldemb)) return -1;
     if (outT && !make_map_ex(&tmT, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (const void*)outT, (N + 63) / 64 * 64, M, ldoT, 32, BN, CU_TENSOR_MAP_SWIZZLE_NONE)) return -1;
     GemmEpi E;
     E.mode = mode; E.relu = relu; E.ones_col = ones_col; E.fm_cols = fm_cols; E.M = M; E.N = N; E.D = D > 0 ? D : 1; E.mn_major = 0;
@@ -751,8 +827,8 @@ int exb_gemm_bf16_nt(uint64_t A, long long lda, uint64_t B, long long ldb, int M
     dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN, splits);
     E.swap = pick_swap(); E.mc = pick_mc((int)grid.y);
     if (E.swap) grid = dim3(grid.y, grid.x, grid.z);
-    cudaError_t err = BN == 128 ? launch_gemm<128>(grid, (cudaStream_t)stream, tmA, tmB, tmO, tmT, E, nkb, per)
-                                : launch_gemm<64>(grid, (cudaStream_t)stream, tmA, tmB, tmO, tmT, E, nkb, per);
+    cudaError_t err = BN == 128 ? launch_gemm<128>(grid, (cudaStream_t)stream, tmA, tmB, tmO, tmT, tmE, E, nkb, per)
+                                : launch_gemm<64>(grid, (cudaStream_t)stream, tmA, tmB, tmO, tmT, tmE, E, nkb, per);
     if (err == cudaSuccess) err = cudaGetLastError();
     if (err != cudaSuccess) { g_gemm_err = std::string("gemm launch: ") + cudaGetErrorString(err); return -1; }
     return 0;
@@ -765,11 +841,11 @@ int exb_gemm_bf16_nt(uint64_t A, long long lda, uint64_t B, long long ldb, int M
 int exb_gemm_bf16_tn(uint64_t A, long long lda, uint64_t B, long long ldb, int M, int N, int K, uint64_t out,
                      long long ldo, int splits, uint64_t stream) {
     if (K % BK != 0 || lda % 8 != 0 || ldb % 8 != 0) { g_gemm_err = "gemm_tn: K %% 64 / ld %% 8 violated"; return -1; }
-    CUtensorMap tmA, tmB, tmO, tmT;
+    CUtensorMap tmA, tmB, tmO, tmT, tmE;
     if (!make_map_ex(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (const void*)A, K, M, lda, 64, BK, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
     if (!make_map_ex(&tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (const void*)B, K, N, ldb, 64, BK, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
     if (!make_map_ex(&tmO, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (const void*)out, M, N, ldo, 32, 32, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
-    tmT = tmO;
+    tmT = tmE = tmO;
     GemmEpi E;
     memset(&E, 0, sizeof(E));
     E.mode = EPI_DW; E.ones_col = -1; E.M = M; E.N = N; E.D = 1; E.mn_major = 1;
@@ -783,8 +859,8 @@ int exb_gemm_bf16_tn(uint64_t A, long long lda, uint64_t B, long long ldb, int M
     dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN, splits);
     E.swap = pick_swap(); E.mc = pick_mc((int)grid.y);
     if (E.swap) grid = dim3(grid.y, grid.x, grid.z);
-    cudaError_t err = BN == 128 ? launch_gemm<128>(grid, (cudaStream_t)stream, tmA, tmB, tmO, tmT, E, nkb, per)
-                                : launch_gemm<64>(grid, (cudaStream_t)stream, tmA, tmB, tmO, tmT, E, nkb, per);
+    cudaError_t err = BN == 128 ? launch_gemm<128>(grid, (cudaStream_t)stream, tmA, tmB, tmO, tmT, tmE, E, nkb, per)
+                                : launch_gemm<64>(grid, (cudaStream_t)stream, tmA, tmB, tmO, tmT, tmE, E, nkb, per);
     if (err == cudaSuccess) err = cudaGetLastError();
     if (err != cudaSuccess) { g_gemm_err = std::string("gemm_tn launch: ") + cudaGetErrorString(err); return -1; }
     return 0;
@@ -842,6 +918,8 @@ void* exb_chain_create(const void* descs, int n, int sms) {
             if (f32out) ok = make_map_ex(&maps[i].tmO, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (const void*)d.out, d.M, d.N, d.ldo, 32, 32, CU_TENSOR_MAP_SWIZZLE_128B);
             else ok = make_map_ex(&maps[i].tmO, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (const void*)d.out, d.M, (d.N + 63) / 64 * 64, d.ldo, 64, 32, CU_TENSOR_MAP_SWIZZLE_128B);
         }
+        if (ok && !d.tn)
+            ok = make_epi_src_map(&maps[i].tmE, E.mode, d.fm_cols, d.M, d.N, (const void*)d.mask, d.ldmask, (const void*)d.emb, d.ldemb);
         if (!ok) return nullptr;
         Q.nkb = d.K / BK;
         int splits = d.tn ? std::max(1, d.splits) : 1;
@@ -861,7 +939,7 @@ void* exb_chain_create(const void* descs, int n, int sms) {
     }
     Chain* c = new Chain();
     c->nprob = n; c->total = item0;
-    c->smem = CH_STAGES * (A_BYTES + CH_B_BYTES) + 4 * 8192 + 2 * CH_STAGES * 8 + CH_MAX_PROB * sizeof(ChainMeta) + 1024;
+    c->smem = CH_STAGES * (A_BYTES + CH_B_BYTES) + 4 * 8192 + (2 * CH_STAGES + 4) * 8 + CH_MAX_PROB * sizeof(ChainMeta) + 1024;
     cudaFuncSetAttribute(exb_gemm_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem);
     cudaFuncSetAttribute(exb_gemm_chain_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     // two CTAs per SM by construction: 2 x (smem + 1 KB reserved) <= 227 KB, and __launch_bounds__(288, 2) keeps

@@ -31,6 +31,9 @@ CUDA_ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
               "-Xptxas", "-v"] + CUDA_ARCH_FLAGS
 CXX_FLAGS = ["-O2", "-std=c++17", "-fPIC", "-Wall", "-Wextra", "-pthread"]
+# fp64 tables (dev_shard.cu) promise results bit-identical to the CPU engine, which the host compiler builds without
+# multiply-add contraction; nvcc would contract a*b + c into an FMA. Off the throughput path, so no contraction there.
+NVCC_FILE_FLAGS = {"dev_shard.cu": ["-fmad=false"]}
 
 
 def _sources(sub, exts):
@@ -98,7 +101,9 @@ def _core_digest():
 
 
 def _cuda_digest():
-    return _hash(_sources("cuda", (".cu",)) + _sources("cuda", (".cuh", ".h")) + _sources("core", (".h",)), NVCC_FLAGS)
+    file_flags = [f + "=" + " ".join(v) for f, v in sorted(NVCC_FILE_FLAGS.items())]
+    return _hash(_sources("cuda", (".cu",)) + _sources("cuda", (".cuh", ".h")) + _sources("core", (".h",)),
+                 NVCC_FLAGS + file_flags)
 
 
 def _up_to_date(lib, digest, force):
@@ -159,11 +164,12 @@ def _build_cuda(force=False, verbose=False):
 
     def compile_one(src):
         obj = os.path.join(_OBJ, os.path.basename(src) + ".o")
-        hd = _hash([src] + [d for d in deps if d.endswith((".cuh", ".h"))], NVCC_FLAGS)
+        flags = NVCC_FLAGS + NVCC_FILE_FLAGS.get(os.path.basename(src), [])
+        hd = _hash([src] + [d for d in deps if d.endswith((".cuh", ".h"))], flags)
         st = obj + ".stamp"
         if not force and os.path.exists(obj) and os.path.exists(st) and open(st).read() == hd:
             return obj
-        _run([NVCC] + NVCC_FLAGS + inc + ["-c", src, "-o", obj], log=obj + ".log")
+        _run([NVCC] + flags + inc + ["-c", src, "-o", obj], log=obj + ".log")
         with open(st, "w") as fh:
             fh.write(hd)
         return obj

@@ -6,7 +6,9 @@
 // tables (fp64 runs at a fraction of the fp32 rate and doubles the bytes per row), so fp64 tables get this small, exact engine instead: every row is [weights | optimizer state] in the
 // reference's own layout (EmbeddingOptimizerVariable.h:141), rows live in an open-addressing slab in HBM, and the
 // verbs are the same four as the CPU oracle's (exb_core.cpp: pull / update / get / set) executed by kernels with the
-// SAME shared math header (exb_math.h) in the same per-row order -- the results are bit-identical to the CPU engine.
+// SAME shared math header (exb_math.h) in the same per-row order, and this file is built without multiply-add
+// contraction (_build.py) -- the results are bit-identical to the CPU engine, except FTRL with learning_rate_power
+// != -0.5: CUDA's pow is not the host libm's.
 // Routing between ranks (unique ids -> owner, NCCL all_to_all) is done by the python layer (backend.py).
 #include <cuda_runtime.h>
 #include <stdint.h>

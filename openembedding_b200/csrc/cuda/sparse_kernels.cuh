@@ -522,6 +522,13 @@ __device__ __noinline__ void apply_rows_slow(const TableDev& T, const PlanDev& P
                                              unsigned long long key, unsigned long long row, unsigned h,
                                              unsigned cnt, int flag, int lane);
 
+// A unique id whose hash-shard insert failed (EXB_ERR_HASH_FULL) is skipped by the apply paths, so its summed
+// gradient would stay in accumulator row h and be added to whichever id the next batch maps to h (the same id
+// retried after a rehash: applied twice). One lane clears the row; cold path, out of line.
+__device__ __noinline__ void clear_acc_row(float* arow, int wstride) {
+    for (int c = 0; c < wstride; ++c) arow[c] = 0.f;
+}
+
 // block-wide exclusive prefix of ceil(cnt/32) over n (<= EXB_MAX_SEG) segments -> s_prefix[0..n]
 __device__ __forceinline__ void block_task_prefix(const unsigned* cnt, int n, int* s_prefix,
                                                   int stride = 1) {
@@ -910,7 +917,10 @@ exb_push_update_kernel(const TableDev* __restrict__ tables, PlanDev P,
                     }
                     hh = (hh + 1) & mask;
                 }
-                if (flag == 0) set_error(P.status, EXB_ERR_HASH_FULL);
+                if (flag == 0) {
+                    set_error(P.status, EXB_ERR_HASH_FULL);
+                    clear_acc_row(P.acc + S.acc_off[pt] + (unsigned long long)h * T.wstride, T.wstride);
+                }
                 row = hh;
             }
             if (flag) ++n_unique_local;

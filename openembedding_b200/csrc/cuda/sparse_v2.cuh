@@ -605,7 +605,10 @@ exb_push2_kernel(const TableDev* __restrict__ tables, PlanDev P, const float* __
                     }
                     hh = (hh + 1) & mask;
                 }
-                if (flag == 0) set_error(P.status, EXB_ERR_HASH_FULL);
+                if (flag == 0) {
+                    set_error(P.status, EXB_ERR_HASH_FULL);
+                    clear_acc_row(L.acc + S.acc_off[pt] + (unsigned long long)h * T.wstride, T.wstride);
+                }
                 row = hh;
             }
             if (flag) ++n_unique_local;

@@ -2,6 +2,7 @@
 
     python benchmarks/step_gemms.py                       # batch 4096, dim 64, hidden (400, 400, 400)
     python benchmarks/step_gemms.py --steps 500 --widths 64,128
+    python benchmarks/step_gemms.py --widths 64 --mc 0,7 --rounds 3     # A-tile multicast off / on, alternated
 
 For every GEMM of the step (fwd1..3, then dX3, dW3, dX2, dW2, dX1 with the FM term, dW1 split-K) this prints, per
 single-launch tile width BN: the time of the single launch (``gemm_nt`` / ``gemm_tn``), the achieved TFLOP/s and the
@@ -16,9 +17,15 @@ whole K range (split-K only cuts that range into pieces), so
 
     bytes = M*K*2 * ceil(N / BN) + N*K*2 * ceil(M / 128)
 
-The single-launch width follows ``EXB_GEMM_BN`` (read once per process), so each width runs in a child process of its
-own. The GEMM shapes depend on batch, dim, hidden and the dense-feature count only, so the embedding tables are kept
-small. Output: one JSON line per measurement, then a markdown table.
+With the A tile multicast to the C CTAs of a cluster (consecutive N tiles), A is read once per cluster: the first
+term becomes M*K*2 * ceil(ceil(N / BN) / C).
+
+The single-launch width follows ``EXB_GEMM_BN`` and the single-launch A-tile multicast ``EXB_GEMM_MC`` (``--mc``: the
+cluster size is the largest divisor of the N-tile count up to that value). Both are read once per process, so each
+combination runs in a child process of its own; with ``--rounds R`` the whole list of combinations runs R times in
+turn, so that the arms are compared under the same drift of a shared card. The GEMM shapes depend on batch, dim,
+hidden and the dense-feature count only, so the embedding tables are kept small. Output: one JSON line per
+measurement, then a markdown table.
 """
 import argparse
 import json
@@ -36,14 +43,21 @@ ap.add_argument("--dim", type=int, default=64)
 ap.add_argument("--steps", type=int, default=300)
 ap.add_argument("--warmup", type=int, default=30)
 ap.add_argument("--widths", default="64,128", help="tile widths to time, comma list")
+ap.add_argument("--mc", default="0", help="EXB_GEMM_MC values to time, comma list (0: no multicast)")
+ap.add_argument("--rounds", type=int, default=1, help="run the list of combinations this many times, alternated")
 ap.add_argument("--child", type=int, default=0, help=argparse.SUPPRESS)   # single-launch width of this process
 a = ap.parse_args()
 
 BM = 128
 
 
-def l2_bytes(M, N, K, bn):
-    return M * K * 2 * math.ceil(N / bn) + N * K * 2 * math.ceil(M / BM)
+def l2_bytes(M, N, K, bn, c=1):
+    return M * K * 2 * math.ceil(math.ceil(N / bn) / c) + N * K * 2 * math.ceil(M / BM)
+
+
+def single_mc(mc, n_tiles):
+    """cluster size of a single launch under EXB_GEMM_MC = mc (gemm_wgmma.cu pick_mc)"""
+    return max([1] + [c for c in range(2, min(mc, 8) + 1) if n_tiles % c == 0])
 
 
 def card():
@@ -57,7 +71,7 @@ def card():
         return torch.cuda.get_device_name(), "unknown"
 
 
-def child(bn):
+def child(bn, mc):
     import torch
     import openembedding_b200 as oe
     from openembedding_b200.context import get_context
@@ -144,15 +158,15 @@ def child(bn):
     name, power = card()
     out = []
     for nm, M, N, K, single, desc in gemms + nofm:
-        row = {"gemm": nm, "M": M, "N": N, "K": K, "bn": bn, "single_us": timed(single)}
+        row = {"gemm": nm, "M": M, "N": N, "K": K, "bn": bn, "mc": mc, "single_us": timed(single)}
         row["chain_us"] = run_chain([desc()])
         row["gflop"] = 2.0 * M * N * K / 1e9
-        row["l2_MB"] = l2_bytes(M, N, K, bn) / 1e6
+        row["l2_MB"] = l2_bytes(M, N, K, bn, single_mc(mc, math.ceil(N / bn))) / 1e6
         row["tflops_single"] = row["gflop"] / row["single_us"] * 1e3
         out.append(row)
 
     fwd_single = timed(lambda: [gm[4]() for gm in gemms[:L]])
-    whole = {"bn": bn, "fwd_3_single_us": fwd_single, "bwd_6_single_us": timed(lambda: [gm[4]() for gm in gemms[L:]])}
+    whole = {"bn": bn, "mc": mc, "fwd_3_single_us": fwd_single, "bwd_6_single_us": timed(lambda: [gm[4]() for gm in gemms[L:]])}
     # whole chains with their dependencies, built as FusedCTR builds them
     fd = []
     for l in range(L):
@@ -168,40 +182,46 @@ def child(bn):
         bd += [dx, dw]
         prod = len(bd) - 2
     whole["bwd_chain_us"] = run_chain(bd)
+    whole["bwd_chain_l2_MB"] = sum(l2_bytes(gm[1], gm[2], gm[3], 64) for gm in gemms[L:]) / 1e6
     print(json.dumps({"card": name, "power_limit": power, "rows": out, "whole": whole}), flush=True)
 
 
 if a.child:
-    child(a.child)
+    child(a.child, int(os.environ.get("EXB_GEMM_MC", "0")))
     sys.exit(0)
 
+ints = lambda s: [int(x) for x in s.split(",")]
+combos = [(w, mc) for w in ints(a.widths) for mc in ints(a.mc)]
 results = []
-for w in (int(x) for x in a.widths.split(",")):
-    env = dict(os.environ, EXB_GEMM_BN=str(w))
-    p = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", str(w), "--batch", str(a.batch),
-                        "--dim", str(a.dim), "--steps", str(a.steps), "--warmup", str(a.warmup)],
-                       env=env, stdout=subprocess.PIPE, text=True)
-    if p.returncode != 0:
-        raise SystemExit("child for BN=%d failed (exit %d)" % (w, p.returncode))
-    r = json.loads(p.stdout.strip().splitlines()[-1])
-    print(json.dumps(r), flush=True)
-    results.append(r)
+for _ in range(a.rounds):
+    for w, mc in combos:
+        env = dict(os.environ, EXB_GEMM_BN=str(w), EXB_GEMM_MC=str(mc))
+        p = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", str(w), "--batch", str(a.batch),
+                            "--dim", str(a.dim), "--steps", str(a.steps), "--warmup", str(a.warmup)],
+                           env=env, stdout=subprocess.PIPE, text=True)
+        if p.returncode != 0:
+            raise SystemExit("child for BN=%d, EXB_GEMM_MC=%d failed (exit %d)" % (w, mc, p.returncode))
+        r = json.loads(p.stdout.strip().splitlines()[-1])
+        print(json.dumps(r), flush=True)
+        results.append(r)
 
 r0 = results[0]
 print("\n%s, power limit %s; batch %d, dim %d; us per launch over %d launches after %d\n"
       % (r0["card"], r0["power_limit"], a.batch, a.dim, a.steps, a.warmup))
 f = lambda v: "%.1f" % v
-print("| GEMM | M x N x K | GFLOP | BN | L2 operand MB | single us | TFLOP/s | one-GEMM chain us |")
-print("|---|---|---|---|---|---|---|---|")
+print("| GEMM | M x N x K | GFLOP | BN | MC | L2 operand MB | single us | TFLOP/s | one-GEMM chain us |")
+print("|---|---|---|---|---|---|---|---|---|")
 for i in range(len(r0["rows"])):
     for r in results:
         x = r["rows"][i]
-        print("| %s | %d x %d x %d | %.2f | %d | %.0f | %s | %.0f | %s |"
-              % (x["gemm"], x["M"], x["N"], x["K"], x["gflop"], x["bn"], x["l2_MB"], f(x["single_us"]),
+        print("| %s | %d x %d x %d | %.2f | %d | %d | %.0f | %s | %.0f | %s |"
+              % (x["gemm"], x["M"], x["N"], x["K"], x["gflop"], x["bn"], x["mc"], x["l2_MB"], f(x["single_us"]),
                  x["tflops_single"], f(x["chain_us"])))
-print("\n| BN | forward: 3 single launches us | forward chain us | backward: 6 single launches us | backward chain us |")
-print("|---|---|---|---|---|")
+print("\n| BN | MC | forward: 3 single launches us | forward chain us | backward: 6 single launches us "
+      "| backward chain L2 operand MB | backward chain us |")
+print("|---|---|---|---|---|---|---|")
 for r in results:
     w = r["whole"]
-    print("| %d | %s | %s | %s | %s |" % (w["bn"], f(w["fwd_3_single_us"]), f(w["fwd_chain_us"]),
-                                         f(w["bwd_6_single_us"]), f(w["bwd_chain_us"])))
+    print("| %d | %d | %s | %s | %s | %.0f | %s |"
+          % (w["bn"], w["mc"], f(w["fwd_3_single_us"]), f(w["fwd_chain_us"]), f(w["bwd_6_single_us"]),
+             w["bwd_chain_l2_MB"], f(w["bwd_chain_us"])))

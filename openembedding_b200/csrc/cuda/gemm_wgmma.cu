@@ -267,6 +267,12 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpi& E, float (&acc)[BN 
     // column pairs issued together, ahead of the math and staging stores of those pairs. At two CTAs per SM a
     // thread has 96 registers; BN = 128 with its 64 accumulators takes fewer pairs at a time.
     constexpr int SG = BN == 64 ? BN / 8 : 2;
+    // BN = 64: the S column n % D of this thread's first pair and the step to the next pair (8 columns on), so one
+    // division per tile instead of two per pair; D is even (host-checked) and n is even, so n % D + 1 < D and a pair
+    // is one float2 load. BN = 128 keeps the per-pair divisions: with this its registers spill 64 bytes instead of 8.
+    const bool fm_tile = mode == EPI_DX_FM && n_blk * BN < fm_cols;
+    const int dcol0 = (BN == 64 && fm_tile) ? (n_blk * BN + 2 * (l & 3)) % D : 0;
+    const int dstep = (BN == 64 && fm_tile) ? 8 % D : 0;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
         const int qrow = (w & 1) * 16 + (l >> 2) + 8 * i;
@@ -276,6 +282,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpi& E, float (&acc)[BN 
         const bool fm_row = mode == EPI_DX_FM && rv && n_blk * BN < fm_cols;
         const float dl = fm_row ? __ldg(E.dlogit + row) : 0.f;
         const float* sb = E.S + (size_t)row * D;
+        int dcol = dcol0;
 #pragma unroll
         for (int j0 = 0; j0 < BN / 8; j0 += SG) {
             float2 s[SG];       // S at the two columns of the pair (the FM term's dimension n % D)
@@ -286,7 +293,13 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpi& E, float (&acc)[BN 
                 // per column pair: n is even and fm_cols = nf * Dp a multiple of 4, so n + 1 < fm_cols as well.
                 // fm_cols need not be a multiple of 32 (nf * Dp = 208 at dim 8): the columns of a partial
                 // 32-column group are embedding columns too and need the FM term
-                if (fm_row && n < fm_cols) s[jj] = make_float2(__ldg(sb + n % D), __ldg(sb + (n + 1) % D));
+                if constexpr (BN == 64) {
+                    if (fm_row && n < fm_cols) s[jj] = __ldg(reinterpret_cast<const float2*>(sb + dcol));
+                    dcol += dstep;
+                    if (dcol >= D) dcol -= D;
+                } else if (fm_row && n < fm_cols) {
+                    s[jj] = make_float2(__ldg(sb + n % D), __ldg(sb + (n + 1) % D));
+                }
             }
 #pragma unroll
             for (int jj = 0; jj < SG; ++jj) {
@@ -718,6 +731,14 @@ bool make_epi_src_map(CUtensorMap* map, int mode, int fm_cols, int M, int N, con
     return make_map_ex(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, p, M, fm_cols, ld, 32, 32, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
+// FM term of EPI_DX_FM: the epilogue reads S a column pair at a time as one float2 (epilogue_tile), so the padded
+// dimension D must be even and S 8-byte aligned
+bool fm_operands_ok(int mode, int fm_cols, int D, uint64_t S) {
+    if (mode != EPI_DX_FM || fm_cols <= 0) return true;
+    if (D < 2 || D % 2 != 0 || (S & 7) != 0) { g_gemm_err = "gemm: the FM term needs an even D and an 8-byte aligned S"; return false; }
+    return true;
+}
+
 // tile width: env EXB_GEMM_BN (64 | 128) overrides
 int pick_swap() {
     static int v = -1;
@@ -764,8 +785,11 @@ cudaError_t launch_gemm(dim3 grid, cudaStream_t stream, const CUtensorMap& tmA, 
 }
 
 // cluster size for the A-tile multicast: the largest divisor (<= EXB_GEMM_MC, <= 8) of the number of N tiles.
-// OFF by default (EXB_GEMM_MC unset / 0): whether the smaller L2 read traffic pays for running the CTAs of a
-// cluster in lock step has not been measured on H100.
+// OFF by default (EXB_GEMM_MC unset / 0): on H100 it makes every GEMM of the DeepFM step slower although it cuts the
+// L2 operand bytes by 42-57% (benchmarks/step_gemms.py --mc, docs/benchmark.md; 400 W card, 3 alternated runs):
+// dX1 without FM operands 32.8-33.1 us off, 51.8-52.3 us at 3 CTAs per cluster; fwd1 21.5-21.7 us off, 35.8-36.4 us
+// at 7. The step's GEMMs are not bound by L2 operand bandwidth, and the lock step of a cluster costs more than the
+// bytes it saves.
 int pick_mc(int n_tiles) {
     static int lim = -1;
     if (lim < 0) { const char* e = getenv("EXB_GEMM_MC"); lim = e ? atoi(e) : 0; }
@@ -798,6 +822,7 @@ int exb_gemm_bf16_nt(uint64_t A, long long lda, uint64_t B, long long ldb, int M
                      long long ldmask, uint64_t dlogit, uint64_t S, uint64_t emb, long long ldemb, int fm_cols, int D,
                      int splits, uint64_t stream, uint64_t dbg) {
     if (K % BK != 0 || lda % 8 != 0 || ldb % 8 != 0) { g_gemm_err = "gemm: K %% 64 / ld %% 8 violated"; return -1; }
+    if (!fm_operands_ok(mode, fm_cols, D, S)) return -1;
     CUtensorMap tmA, tmB;
     if (!make_map(&tmA, (const void*)A, M, K, lda, BM)) return -1;
     const int BN = pick_bn(M, N, K);
@@ -899,6 +924,7 @@ void* exb_chain_create(const void* descs, int n, int sms) {
         ChainMeta& Q = meta[i];
         memset(&Q, 0, sizeof(Q));
         if (d.K % BK != 0 || d.lda % 8 != 0 || d.ldb % 8 != 0) { g_gemm_err = "chain: K % 64 / ld % 8 violated"; return nullptr; }
+        if (!d.tn && !fm_operands_ok(d.mode, d.fm_cols, d.D, d.S)) return nullptr;
         GemmEpi& E = Q.E;
         E.mode = d.tn ? EPI_DW : d.mode; E.relu = d.relu; E.ones_col = d.tn ? -1 : d.ones_col; E.fm_cols = d.fm_cols;
         E.M = d.M; E.N = d.N; E.D = d.D > 0 ? d.D : 1; E.mn_major = d.tn ? 1 : 0;

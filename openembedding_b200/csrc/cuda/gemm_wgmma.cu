@@ -505,7 +505,6 @@ constexpr int CH_STAGES = 3;                  // 3 x 24 KB ring + 32 KB epilogue
 constexpr int CH_BN = 64;
 constexpr int CH_B_BYTES = CH_BN * BK * 2;
 constexpr int CH_MAX_PROB = 8;
-constexpr int CH_MAX_MB = 64;                 // row blocks per problem tracked by the ready counters
 
 struct ChainMaps { CUtensorMap tmA, tmB, tmO, tmE; };  // tmE: epilogue source tile (zeroed when the GEMM has none)
 struct ChainMapsAll { ChainMaps m[CH_MAX_PROB]; };    // passed as a __grid_constant__ parameter (4 KB): descriptors in param space
@@ -535,9 +534,11 @@ __device__ __forceinline__ unsigned ch_ld_acquire(const unsigned* p) {
     return v;
 }
 
+// ready: one counter per (GEMM p, row block m) at p * mb_stride + m (mb_stride: the largest row-block count of the
+// chain), then the counter of CTAs that have left
 __global__ void __launch_bounds__(NUM_THREADS, 2)
 exb_gemm_chain_kernel(const __grid_constant__ ChainMapsAll MAPS, const ChainMeta* __restrict__ metas, int nprob, int total_items,
-                      unsigned* __restrict__ ready, int* __restrict__ err) {
+                      unsigned* __restrict__ ready, int mb_stride, int* __restrict__ err) {
     const ChainMaps* maps = MAPS.m;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -575,7 +576,7 @@ exb_gemm_chain_kernel(const __grid_constant__ ChainMapsAll MAPS, const ChainMeta
                 if (Q.dep_kind) {      // the row blocks this tile reads must be complete
                     int mb0 = m_blk, mb1 = m_blk + 1;
                     if (Q.dep_kind == 2) { mb0 = (kb0 * BK) / BM; mb1 = (kb1 * BK + BM - 1) / BM; }
-                    const unsigned* cnt = ready + Q.dep * CH_MAX_MB;
+                    const unsigned* cnt = ready + Q.dep * mb_stride;
                     for (int mb = mb0; mb < mb1; ++mb) {
                         uint32_t it = 0;
                         while (ch_ld_acquire(cnt + mb) < (unsigned)Q.dep_need) {
@@ -641,7 +642,7 @@ exb_gemm_chain_kernel(const __grid_constant__ ChainMapsAll MAPS, const ChainMeta
                     asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
                     asm volatile("fence.proxy.async;" ::: "memory");
                     __threadfence();
-                    atomicAdd(&ready[p * CH_MAX_MB + m_blk], 1u);
+                    atomicAdd(&ready[p * mb_stride + m_blk], 1u);
                 } else {
                     // nobody inside this launch reads the tile (dW, the last dX): only the staging tile has to be free
                     // again; kernel completion makes the writes visible to the next kernel
@@ -656,16 +657,17 @@ exb_gemm_chain_kernel(const __grid_constant__ ChainMapsAll MAPS, const ChainMeta
     // self-cleaning dependency counters: the LAST CTA to leave zeroes them for the next launch (no memset node in
     // front of the kernel, so the launch keeps its programmatic-dependent-launch edge inside a CUDA graph)
     if (warp == 0) {
+        const int ncnt = nprob * mb_stride;
         unsigned last = 0;
         if (lane == 0) {
             __threadfence();
-            last = (atomicAdd(&ready[CH_MAX_PROB * CH_MAX_MB], 1u) == gridDim.x - 1) ? 1u : 0u;
+            last = (atomicAdd(&ready[ncnt], 1u) == gridDim.x - 1) ? 1u : 0u;
         }
         last = __shfl_sync(0xffffffffu, last, 0);
         if (last) {
-            for (int i = lane; i < CH_MAX_PROB * CH_MAX_MB; i += 32) ready[i] = 0u;
+            for (int i = lane; i < ncnt; i += 32) ready[i] = 0u;
             __syncwarp();
-            if (lane == 0) { __threadfence(); ready[CH_MAX_PROB * CH_MAX_MB] = 0u; }
+            if (lane == 0) { __threadfence(); ready[ncnt] = 0u; }
         }
     }
 }
@@ -816,12 +818,14 @@ int exb_gemm_timeouts() {
 }
 
 // D (+)= A[M,K](lda) * B[N,K](ldb)^T, bf16 in. K must be a multiple of 64 (pad the operands);
-// lda/ldb in elements, multiples of 8. epi: see GemmEpi. splits >= 1 (EPI_DW only).
+// lda/ldb in elements, multiples of 8. epi: see GemmEpi. splits > 1: EPI_DW only (the other epilogues store their
+// tile, so the K splits would overwrite each other's partial sums).
 int exb_gemm_bf16_nt(uint64_t A, long long lda, uint64_t B, long long ldb, int M, int N, int K, int mode, int relu,
                      int ones_col, uint64_t out, long long ldo, uint64_t outT, long long ldoT, uint64_t mask,
                      long long ldmask, uint64_t dlogit, uint64_t S, uint64_t emb, long long ldemb, int fm_cols, int D,
                      int splits, uint64_t stream, uint64_t dbg) {
     if (K % BK != 0 || lda % 8 != 0 || ldb % 8 != 0) { g_gemm_err = "gemm: K %% 64 / ld %% 8 violated"; return -1; }
+    if (splits > 1 && mode != EPI_DW) { g_gemm_err = "gemm: splits > 1 needs EPI_DW (split-K sums are reduce-added)"; return -1; }
     if (!fm_operands_ok(mode, fm_cols, D, S)) return -1;
     CUtensorMap tmA, tmB;
     if (!make_map(&tmA, (const void*)A, M, K, lda, BM)) return -1;
@@ -903,7 +907,7 @@ struct ChainDesc {      // one GEMM of a chain (python: ops/gemm.py ChainDesc)
     int dep, dep_kind;  // index of the GEMM of this chain that produces this one's A operand (-1: none); kind 1 row block, 2 K range
 };
 struct Chain {
-    int nprob = 0, total = 0, grid = 0;
+    int nprob = 0, total = 0, grid = 0, mb_stride = 1;
     ChainMapsAll maps;
     ChainMeta* d_meta = nullptr;
     unsigned* d_ready = nullptr;
@@ -958,13 +962,22 @@ void* exb_chain_create(const void* descs, int n, int sms) {
         Q.dep = d.dep; Q.dep_kind = d.dep >= 0 ? d.dep_kind : 0; Q.dep_need = 0; Q.signal = 0;
         if (Q.dep_kind) {
             if (d.dep >= i) { g_gemm_err = "chain: a GEMM may only depend on an earlier one"; return nullptr; }
+            // the row blocks a tile waits on must be row blocks its producer writes: the counters of the next GEMM
+            // (or past the table) would otherwise be read as this producer's
+            const int rows_read = Q.dep_kind == 1 ? Q.m_tiles : Q.dep_kind == 2 ? (d.K + BM - 1) / BM : -1;
+            if (rows_read < 0 || rows_read > meta[d.dep].m_tiles) {
+                g_gemm_err = "chain: a dependency reads row blocks its producer does not write";
+                return nullptr;
+            }
             meta[d.dep].signal = 1;
             Q.dep_need = (NUM_CONSUMER_WARPS / 4) * meta[d.dep].n_tiles;   // each consumer warpgroup signs off every tile of the row block
-            if (meta[d.dep].m_tiles > CH_MAX_MB) { g_gemm_err = "chain: too many row blocks"; return nullptr; }
         }
     }
+    int mb_stride = 1;     // ready counters per GEMM: its row blocks (the largest count of the chain)
+    for (int i = 0; i < n; ++i) mb_stride = std::max(mb_stride, meta[i].m_tiles);
+    const size_t ready_bytes = ((size_t)n * mb_stride + 1) * sizeof(unsigned);
     Chain* c = new Chain();
-    c->nprob = n; c->total = item0;
+    c->nprob = n; c->total = item0; c->mb_stride = mb_stride;
     c->smem = CH_STAGES * (A_BYTES + CH_B_BYTES) + 4 * 8192 + (2 * CH_STAGES + 4) * 8 + CH_MAX_PROB * sizeof(ChainMeta) + 1024;
     cudaFuncSetAttribute(exb_gemm_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem);
     cudaFuncSetAttribute(exb_gemm_chain_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
@@ -978,11 +991,11 @@ void* exb_chain_create(const void* descs, int n, int sms) {
     memset(&c->maps, 0, sizeof(c->maps));
     for (int i = 0; i < n; ++i) c->maps.m[i] = maps[i];
     if (cudaMalloc(&c->d_meta, n * sizeof(ChainMeta)) != cudaSuccess ||
-        cudaMalloc(&c->d_ready, (CH_MAX_PROB * CH_MAX_MB + 32) * 4) != cudaSuccess || cudaMalloc(&c->d_err, 4) != cudaSuccess) {
+        cudaMalloc(&c->d_ready, ready_bytes) != cudaSuccess || cudaMalloc(&c->d_err, 4) != cudaSuccess) {
         g_gemm_err = "chain: cudaMalloc failed"; delete c; return nullptr;
     }
     cudaMemcpy(c->d_meta, meta.data(), n * sizeof(ChainMeta), cudaMemcpyHostToDevice);
-    cudaMemset(c->d_ready, 0, (CH_MAX_PROB * CH_MAX_MB + 32) * 4);
+    cudaMemset(c->d_ready, 0, ready_bytes);
     cudaMemset(c->d_err, 0, 4);
     return c;
 }
@@ -994,7 +1007,7 @@ void exb_chain_destroy(void* h) {
 int exb_chain_launch(void* h, uint64_t stream) {
     Chain* c = (Chain*)h;
     cudaError_t err = exb::launch_pdl(exb_gemm_chain_kernel, dim3(c->grid), dim3(NUM_THREADS), c->smem, (cudaStream_t)stream,
-                              c->maps, (const ChainMeta*)c->d_meta, c->nprob, c->total, c->d_ready, c->d_err);
+                              c->maps, (const ChainMeta*)c->d_meta, c->nprob, c->total, c->d_ready, c->mb_stride, c->d_err);
     if (err == cudaSuccess) err = cudaGetLastError();
     if (err != cudaSuccess) { g_gemm_err = std::string("chain launch: ") + cudaGetErrorString(err); return -1; }
     return 0;

@@ -3,6 +3,10 @@
 ``gemm_nt(A, B, ...)`` computes ``A[M,K] @ B[N,K].T`` on bf16 operands with one of the
 fused epilogues. Operands must be K-padded to a multiple of 64 and have leading
 dimensions that are multiples of 8 elements (the dense engine allocates them that way).
+
+Outputs are stored by TMA in whole 16-byte units of a row: when an output row (or a row of ``outT``) is not a
+multiple of 16 bytes wide, the elements up to the next 16-byte boundary, inside the row stride, are overwritten too.
+``splits > 1`` is for EPI_DW only (split-K partial sums are reduce-added); other epilogues refuse it.
 """
 import ctypes
 from ctypes import c_int, c_longlong, c_uint64

@@ -37,6 +37,7 @@ ap.add_argument("--cpu", action="store_true")
 ap.add_argument("--checkpoint", default="")
 ap.add_argument("--load", default="")
 ap.add_argument("--save", default="")
+ap.add_argument("--export", default="", help="with --fused: stand-alone PyTorch model file (no engine, no GPU needed)")
 args = ap.parse_args()
 
 world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -63,6 +64,8 @@ label = torch.tensor(part["label"].values, dtype=torch.float32)
 
 if args.validation_batches and not args.fused:
     raise SystemExit("--validation_batches: evaluation runs on the fused step (--fused)")
+if args.export and not args.fused:
+    raise SystemExit("--export: the stand-alone export is of the fused models (--fused)")
 n_val = args.validation_batches * args.batch_size
 if n_val >= n:
     raise SystemExit("--validation_batches %d leaves no training batch" % args.validation_batches)
@@ -83,7 +86,10 @@ else:
                      compute_dtype=torch.float32 if ctx.device.type == "cpu" else torch.bfloat16)
     trainer = Trainer(model, use_graph=False)
 if args.load:
-    embed.load_server_model(model, args.load)
+    if args.fused:               # dense weights, dense optimizer and the tables
+        model.load(args.load)
+    else:
+        embed.load_server_model(model, args.load)
 for epoch in range(args.epochs):
     tot, cnt = 0.0, 0
     for i in range(0, n_train, args.batch_size):
@@ -103,10 +109,18 @@ for epoch in range(args.epochs):
         r = metrics.result()                # all ranks: the counters are summed over them
         if ctx.rank == 0:
             print("epoch %d val_auc %.4f val_logloss %.4f" % (epoch + 1, r["auc"], r["logloss"]))
-    if args.checkpoint:
-        embed.save_server_model(model, args.checkpoint + str(epoch + 1))          # include optimizer
+    if args.checkpoint:                                                            # include optimizer
+        if args.fused:
+            model.save(args.checkpoint + str(epoch + 1))
+        else:
+            embed.save_server_model(model, args.checkpoint + str(epoch + 1))
 if args.save:
-    embed.save_server_model(model, args.save, include_optimizer=False)
+    if args.fused:
+        model.save(args.save, include_optimizer=False)
+    else:
+        embed.save_server_model(model, args.save, include_optimizer=False)
+if args.export:
+    model.save_as_original_model(args.export)
 if world > 1:
     dist.barrier()
     dist.destroy_process_group()

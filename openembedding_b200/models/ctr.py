@@ -181,7 +181,68 @@ class CrossNetV2(nn.Module):
         return x
 
 
-class CTRModel(nn.Module):
+class _CTRHead(nn.Module):
+    """The dense part of the zoo's CTR models, shared by ``CTRModel`` and ``StandaloneCTR``: the layers after the
+    row lookup, and the logit from the looked-up rows."""
+
+    def _build_dense(self, num_dense, dnn_hidden, tc, cin_layers, cross_layers, cin_split_half=True):
+        """dense_linear, bias and (models with embeddings) dnn, dnn_out, cin / cin_out, cross"""
+        nf, embedding_dim = self.nf, self.D
+        dnn_in = nf * embedding_dim + num_dense
+        self.tc = tc
+        Linear, _ = _gemm_layers(tc)
+        self.dense_linear = nn.Linear(num_dense, 1, bias=False) if num_dense else None
+        self.bias = nn.Parameter(torch.zeros(1))
+        layers, prev = [], dnn_in
+        if self.has_emb:
+            for h in dnn_hidden:
+                layers += [Linear(prev, h), nn.ReLU()]
+                prev = h
+            self.dnn = nn.Sequential(*layers)
+            self.dnn_out = nn.Linear(prev, 1, bias=False)
+        if self.model_name == "xdeepfm":
+            self.cin = CIN(nf, cin_layers, split_half=cin_split_half, tc=tc)
+            self.cin_out = nn.Linear(self.cin.out_dim, 1, bias=False)
+        if self.model_name == "dcn":
+            self.cross = CrossNetV2(dnn_in, cross_layers, tc=tc)
+            self.dnn_out = nn.Linear(prev + dnn_in, 1, bias=False)
+
+    def _cached_rows(self, ids, embs, lins):
+        """append the rows of the replicated ("cache") tables to the embedding / linear parts"""
+        if self.cached:
+            cid = ids[:, self.cache_cols] + self.cache_offsets            # [B, nc]
+            if self.has_emb:
+                embs.append(_GatherRows.apply(self.cache_emb, cid))
+            lins.append(_GatherRows.apply(self.cache_lin, cid).squeeze(-1))
+
+    def _logit(self, embs, lins, dense):
+        """logits [B] from the embedding parts ([B, n, D] each; server features, then cached ones), the linear
+        parts ([B, n] each) and the dense input"""
+        linear = torch.cat(lins, dim=1).sum(dim=1)
+        if self.dense_linear is not None:
+            linear = linear + self.dense_linear(dense).squeeze(-1)
+        logit = linear + self.bias
+        if not self.has_emb:
+            return logit
+        B = dense.shape[0]
+        emb = torch.cat(embs, dim=1) if len(embs) > 1 else embs[0]        # [B, nf, D] fp32
+        with torch.autocast(device_type=emb.device.type, dtype=self.compute_dtype,
+                            enabled=self.compute_dtype != torch.float32 and not self.tc):
+            x = torch.cat([emb.reshape(B, -1), dense], dim=1)
+            if self.model_name == "dcn":
+                h = torch.cat([self.cross(x), self.dnn(x)], dim=1)
+                logit = logit + self.dnn_out(h).squeeze(-1).float()
+            else:
+                logit = logit + self.dnn_out(self.dnn(x)).squeeze(-1).float()
+            if self.model_name == "xdeepfm":
+                logit = logit + self.cin_out(self.cin(emb)).squeeze(-1).float()
+        if self.model_name == "deepfm":
+            s = emb.sum(dim=1)
+            logit = logit + 0.5 * (s * s - (emb * emb).sum(dim=1)).sum(dim=1)
+        return logit
+
+
+class CTRModel(_CTRHead):
     """model in {"lr", "wdl", "deepfm", "xdeepfm", "dcn"}"""
 
     def __init__(self, vocab_sizes, num_dense=13, embedding_dim=9, model="deepfm", batch=4096,
@@ -226,26 +287,9 @@ class CTRModel(nn.Module):
             self.register_buffer("cache_cols", torch.tensor(self.cached, dtype=torch.int64, device=ctx.device))
             self.cache_emb = nn.Parameter(torch.zeros(off, embedding_dim, device=ctx.device)) if self.has_emb else None
             self.cache_lin = nn.Parameter(torch.zeros(off, 1, device=ctx.device))
-        dnn_in = nf * embedding_dim + num_dense
         # GEMM-shaped layers on the hand-written wgmma kernel (bf16 operands) when the model computes in bf16 on CUDA
         tc = ctx.device.type == "cuda" and compute_dtype == torch.bfloat16
-        self.tc = tc
-        Linear, _ = _gemm_layers(tc)
-        self.dense_linear = nn.Linear(num_dense, 1, bias=False) if num_dense else None
-        self.bias = nn.Parameter(torch.zeros(1))
-        layers, prev = [], dnn_in
-        if self.has_emb:
-            for h in dnn_hidden:
-                layers += [Linear(prev, h), nn.ReLU()]
-                prev = h
-            self.dnn = nn.Sequential(*layers)
-            self.dnn_out = nn.Linear(prev, 1, bias=False)
-        if self.model_name == "xdeepfm":
-            self.cin = CIN(nf, cin_layers, tc=tc)
-            self.cin_out = nn.Linear(self.cin.out_dim, 1, bias=False)
-        if self.model_name == "dcn":
-            self.cross = CrossNetV2(dnn_in, cross_layers, tc=tc)
-            self.dnn_out = nn.Linear(prev + dnn_in, 1, bias=False)
+        self._build_dense(num_dense, dnn_hidden, tc, cin_layers, cross_layers)
         self.to(ctx.device)
 
     def dense_parameters(self):
@@ -265,32 +309,50 @@ class CTRModel(nn.Module):
                 embs.append(out[:, s0:s0 + ns * es].reshape(B, ns, es)[:, :, :self.D])
             l0 = self._lin_slices[0].start
             lins.append(out[:, l0:l0 + len(self.server)])
+        self._cached_rows(ids, embs, lins)
+        return self._logit(embs, lins, dense)
+
+
+class StandaloneCTR(_CTRHead):
+    """A trained Wide&Deep / DeepFM / xDeepFM / DCN-v2 as a plain fp32 module that needs no engine and no GPU (the
+    export of ``FusedCTR.save_as_original_model``): ``emb[j]`` (dim D) and ``lin[j]`` (dim 1) are the
+    ``nn.Embedding`` tables of the j-th server feature, ``cache_emb`` / ``cache_lin`` the replicated tables of the
+    ``cached`` features, and the dense layers carry ``CTRModel``'s names. ``forward(ids [B, nf], dense [B, nd])``
+    returns fp32 logits [B]."""
+
+    def __init__(self, vocab_sizes, num_dense=13, embedding_dim=9, model="deepfm", hidden=None, cached=(),
+                 cin_layers=(128, 128), cin_split_half=True, cross_layers=3):
+        super().__init__()
+        self.model_name = model.lower()
+        if self.model_name not in ("wdl", "deepfm", "xdeepfm", "dcn"):
+            raise ValueError("StandaloneCTR: wdl, deepfm, xdeepfm or dcn")
+        self.num_dense, self.D = num_dense, embedding_dim
+        self.vocab_sizes = list(vocab_sizes)
+        self.nf = nf = len(self.vocab_sizes)
+        self.compute_dtype, self.has_emb = torch.float32, True
+        if hidden is None:
+            hidden = (512, 256, 128, 32) if self.model_name == "wdl" else (400, 400, 400)
+        self.cached = list(cached)
+        self.server = [f for f in range(nf) if f not in self.cached]
+        self.emb = nn.ModuleList([nn.Embedding(self.vocab_sizes[f], embedding_dim) for f in self.server])
+        self.lin = nn.ModuleList([nn.Embedding(self.vocab_sizes[f], 1) for f in self.server])
         if self.cached:
-            cid = ids[:, self.cache_cols] + self.cache_offsets            # [B, nc]
-            if self.has_emb:
-                embs.append(_GatherRows.apply(self.cache_emb, cid))
-            lins.append(_GatherRows.apply(self.cache_lin, cid).squeeze(-1))
-        linear = torch.cat(lins, dim=1).sum(dim=1)
-        if self.dense_linear is not None:
-            linear = linear + self.dense_linear(dense).squeeze(-1)
-        logit = linear + self.bias
-        if not self.has_emb:
-            return logit
-        emb = torch.cat(embs, dim=1) if len(embs) > 1 else embs[0]        # [B, nf, D] fp32
-        with torch.autocast(device_type=emb.device.type, dtype=self.compute_dtype,
-                            enabled=self.compute_dtype != torch.float32 and not self.tc):
-            x = torch.cat([emb.reshape(B, -1), dense], dim=1)
-            if self.model_name == "dcn":
-                h = torch.cat([self.cross(x), self.dnn(x)], dim=1)
-                logit = logit + self.dnn_out(h).squeeze(-1).float()
-            else:
-                logit = logit + self.dnn_out(self.dnn(x)).squeeze(-1).float()
-            if self.model_name == "xdeepfm":
-                logit = logit + self.cin_out(self.cin(emb)).squeeze(-1).float()
-        if self.model_name == "deepfm":
-            s = emb.sum(dim=1)
-            logit = logit + 0.5 * (s * s - (emb * emb).sum(dim=1)).sum(dim=1)
-        return logit
+            offs = [sum(self.vocab_sizes[g] for g in self.cached[:i]) for i in range(len(self.cached))]
+            rows = sum(self.vocab_sizes[f] for f in self.cached)
+            self.register_buffer("cache_offsets", torch.tensor(offs, dtype=torch.int64))
+            self.register_buffer("cache_cols", torch.tensor(self.cached, dtype=torch.int64))
+            self.cache_emb = nn.Parameter(torch.zeros(rows, embedding_dim))
+            self.cache_lin = nn.Parameter(torch.zeros(rows, 1))
+        self._build_dense(num_dense, hidden, False, cin_layers, cross_layers, cin_split_half)
+
+    def forward(self, ids, dense):
+        embs, lins = [], []
+        if self.server:
+            embs.append(torch.stack([t(ids[:, f]) for t, f in zip(self.emb, self.server)], dim=1))
+            lins.append(torch.cat([t(ids[:, f]) for t, f in zip(self.lin, self.server)], dim=1))
+        self._cached_rows(ids, embs, lins)
+        return self._logit(embs, lins, dense)
+
 
 class CriteoLR(nn.Module):
     """examples/criteo_lr_subclass.py: ONE hashed dim-1 table shared by all 26 sparse

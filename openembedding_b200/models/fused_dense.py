@@ -33,6 +33,7 @@ prep, the forward GEMMs, the CIN / cross forward and the predict head (logits + 
 import ctypes
 import os
 import math
+import shutil
 from ctypes import c_float, c_int, c_longlong, c_void_p
 
 import torch
@@ -234,6 +235,122 @@ def cin_dims(nf, cin_layers, split_half):
     return H, layers, Kp, Np, dir_lo
 
 
+class DenseLayout:
+    """What ``FusedCTR``'s flat padded fp32 buffer (``theta``, and alike ``gtheta`` / ``accum`` / ``accum2``) holds.
+
+    ``segs``    {segment: (offset, size)}, ``n_theta`` the buffer's length;
+    ``shapes``  {segment: (R, C)}: the DNN / CIN / cross matrices ``W{l}`` / ``C{k}`` / ``X{l}`` are [R, C], the
+                replicated table ``cache_emb`` is [rows, Dp], every other segment is one row of C entries;
+    ``params``  {logical name: (shape, blocks)}: a block (segment, rows, cols) is the sub-matrix of real rows and
+                columns of one segment; a parameter is its blocks side by side, reshaped to ``shape``.
+
+    The logical names and shapes are those of ``models.ctr.CTRModel``'s dense parameters, plus ``dnn_out.bias``
+    (the output weight that faces the last hidden layer's ones column). The embedding columns of the first DNN
+    layer and of the cross network are in the order server features, then cached features (the A0 order)."""
+
+    def __init__(self, segs, n_theta, shapes, params):
+        self.segs, self.n_theta, self.shapes, self.params = segs, n_theta, shapes, params
+
+    def index(self, name):
+        """flat indices (int64, the parameter's shape) of a logical parameter in the buffer"""
+        def ix(v):
+            return torch.arange(v.start, v.stop) if isinstance(v, range) else torch.as_tensor(v, dtype=torch.long)
+
+        shape, blocks = self.params[name]
+        parts = []
+        for seg, rows, cols in blocks:
+            off, C = self.segs[seg][0], self.shapes[seg][1]
+            parts.append(off + ix(rows)[:, None] * C + ix(cols)[None, :])
+        return torch.cat(parts, 1).reshape(shape)
+
+    def gather(self, flat):
+        """{logical name: tensor} read out of a flat buffer"""
+        return {name: flat[self.index(name).to(flat.device)] for name in self.params}
+
+    def scatter(self, flat, tensors):
+        """write every logical parameter of ``tensors`` into the flat buffer (in place)"""
+        for name in self.params:
+            idx = self.index(name).to(flat.device)
+            flat[idx] = tensors[name].to(device=flat.device, dtype=flat.dtype).reshape(idx.shape)
+
+
+def dense_layout(vocab_sizes, num_dense, embedding_dim, model, hidden, cached=(), cin_layers=(128, 128),
+                 cin_split_half=True, cross_layers=3):
+    """The ``DenseLayout`` of a ``FusedCTR`` configuration (``cached``: the features held in the replicated table).
+    Needs no GPU: save, load and export read and write the dense state through this map alone."""
+    vocab, model, hidden = list(vocab_sizes), model.lower(), [int(h) for h in hidden]
+    nf, nd, D, Dp = len(vocab), int(num_dense), int(embedding_dim), _r(int(embedding_dim), 4)
+    Hp = [_r(h + 1, 64) for h in hidden]
+    K0p = _r(nf * Dp + nd + 1, 64)
+    dims = [K0p] + Hp
+    segs, shapes, off = {}, {}, 0
+
+    def seg(name, R, C, n=None):
+        nonlocal off
+        segs[name], shapes[name] = (off, R * C), (R, C)
+        off = _r(off + (R * C if n is None else n), 4)
+
+    for l in range(len(hidden)):
+        seg("W%d" % l, Hp[l], dims[l])
+    cin = model == "xdeepfm"
+    if cin:
+        cH, cN, cKp, cNp, clo = cin_dims(nf, cin_layers, cin_split_half)
+        for k in range(len(cN)):        # bias in column H_k * nf
+            seg("C%d" % k, cNp[k], cKp[k])
+    Lc = int(cross_layers) if model == "dcn" else 0
+    for l in range(Lc):                 # bias in the ones column K0p - 1
+        seg("X%d" % l, K0p, K0p)
+    seg("wout", 1, Hp[-1])
+    seg("wd", 1, max(nd, 1))
+    seg("bias", 1, 1)
+    if cin:
+        T = sum(n - lo for n, lo in zip(cN, clo))
+        seg("wcin", 1, T)
+    if Lc:
+        seg("wcross", 1, K0p)
+    vc = sum(vocab[f] for f in cached)
+    seg("cache_emb", vc, Dp)
+    seg("cache_lin", 1, vc, n=max(vc, 1))
+
+    real0 = cross_cols(nf, D, Dp, nd)   # [emb (nf*D) | dense (nd)] among the A0 columns
+    params = {}
+    for l, h in enumerate(hidden):
+        cols = real0 if l == 0 else range(hidden[l - 1])
+        params["dnn.%d.weight" % (2 * l)] = ((h, len(cols)), [("W%d" % l, range(h), cols)])
+        params["dnn.%d.bias" % (2 * l)] = ((h,), [("W%d" % l, range(h), [dims[l] - 1])])
+    hL = hidden[-1]
+    if Lc:                              # CTRModel's order: cat([cross(x), dnn(x)])
+        params["dnn_out.weight"] = ((1, len(real0) + hL), [("wcross", [0], real0), ("wout", [0], range(hL))])
+    else:
+        params["dnn_out.weight"] = ((1, hL), [("wout", [0], range(hL))])
+    params["dnn_out.bias"] = ((1,), [("wout", [0], [Hp[-1] - 1])])
+    if nd:
+        params["dense_linear.weight"] = ((1, nd), [("wd", [0], range(nd))])
+    params["bias"] = ((1,), [("bias", [0], [0])])
+    if vc:
+        params["cache_emb"] = ((vc, D), [("cache_emb", range(vc), range(D))])
+        params["cache_lin"] = ((vc, 1), [("cache_lin", [0], range(vc))])
+    if cin:
+        for k, n in enumerate(cN):
+            C = cH[k] * nf
+            params["cin.convs.%d.weight" % k] = ((n, C, 1), [("C%d" % k, range(n), range(C))])
+            params["cin.convs.%d.bias" % k] = ((n,), [("C%d" % k, range(n), [C])])
+        params["cin_out.weight"] = ((1, T), [("wcin", [0], range(T))])
+    for l in range(Lc):
+        n = len(real0)
+        params["cross.w.%d.weight" % l] = ((n, n), [("X%d" % l, real0, real0)])
+        params["cross.w.%d.bias" % l] = ((n,), [("X%d" % l, real0, [K0p - 1])])
+    return DenseLayout(segs, off, shapes, params)
+
+
+# the dense optimizer's state slots: accum holds the first, accum2 the second (csrc/cuda/dense_kernels.cu: dense_opt_one)
+DENSE_OPT_SLOTS = {"adagrad": ("accumulator",), "adam": ("m", "v"), "ftrl": ("accumulator", "linear")}
+CHECKPOINT_FORMAT = "openembedding_b200.FusedCTR/1"
+# what a checkpoint must agree on with the model that loads it (batch, world size and optimizer may differ)
+CONFIG_KEYS = ("model", "vocab", "cached", "embedding_dim", "num_dense", "hidden", "cin_layers", "cin_split_half",
+               "cross_layers", "pack_linear")
+
+
 class FusedCTR:
     """DeepFM (use_fm=True), Wide&Deep, xDeepFM or DCN-v2 (use_fm=False; xDeepFM adds the CIN branch, DCN-v2 the
     cross network) with the whole step on own kernels."""
@@ -310,38 +427,19 @@ class FusedCTR:
         self.group = self.sparse.group
         dev = self.dev
         f32, bf16 = torch.float32, torch.bfloat16
-        # ---- flat parameter buffer
-        segs, off = {}, 0
+        # ---- flat parameter buffer: the matrices (DNN, CIN filters [Np_k, Kp_k], cross [K0p, K0p]; refreshed to bf16
+        # by the optimizer), then wout, wd, bias, wcin, wcross (x_L's output weights, zero outside the real columns),
+        # cache_emb, cache_lin (dense_layout)
+        self.layout = dense_layout(self.vocab, num_dense, embedding_dim, self.model, self.hidden, self.cached,
+                                   self.cin_layers, self.cin_split_half, self.cross_layers)
+        segs, off = self.layout.segs, self.layout.n_theta
         dims = [self.K0p] + self.Hp
-        for l in range(len(self.hidden)):
-            n = self.Hp[l] * dims[l]
-            segs["W%d" % l] = (off, n)
-            off = _r(off + n, 4)
         L = len(self.hidden)
         K = len(self.cin_layers)
-        for k in range(K):          # CIN filters [Np_k, Kp_k], bias in column H_k * nf: refreshed matrices as well
-            n = self.cin_Np[k] * self.cin_Kp[k]
-            segs["C%d" % k] = (off, n)
-            off = _r(off + n, 4)
         Lc = self.cross_layers
-        for l in range(Lc):         # cross matrices [K0p, K0p], bias in the ones column: refreshed matrices as well
-            segs["X%d" % l] = (off, self.K0p * self.K0p)
-            off = _r(off + self.K0p * self.K0p, 4)
-        flat = [("wout", self.Hp[-1]), ("wd", max(num_dense, 1)), ("bias", 1)]
         if self.cin:
             self.cin_T = sum(n - lo for n, lo in zip(self.cin_layers, self.cin_lo))    # pooled CIN features
-            flat.append(("wcin", self.cin_T))
-        if self.dcn:
-            flat.append(("wcross", self.K0p))        # x_L's output weights, zero outside the real columns
-        for name, n in flat:
-            segs[name] = (off, n)
-            off = _r(off + n, 4)
-        vc = sum(self.vocab[f] for f in self.cached)
-        self.cache_rows = vc
-        segs["cache_emb"] = (off, vc * Dp)
-        off = _r(off + vc * Dp, 4)
-        segs["cache_lin"] = (off, vc)
-        off = _r(off + max(vc, 1), 4)
+        self.cache_rows = sum(self.vocab[f] for f in self.cached)
         self.segs, self.n_theta = segs, off
         self.theta = torch.zeros(off, dtype=f32, device=dev)
         # dense optimizer (tf.keras semantics): {"category": "adagrad" | "adam" | "ftrl", ...}; default Adagrad(lr)
@@ -353,6 +451,7 @@ class FusedCTR:
         self.dense_opt = dopt
         self.lr = lr = float(dopt["learning_rate"])
         acc0 = float(dopt.get("initial_accumulator_value", 0.0)) if dopt["category"] in ("adagrad", "ftrl") else 0.0
+        self._acc0 = acc0
         self.accum = torch.full((off,), acc0, dtype=f32, device=dev)
         self.accum2 = torch.zeros(off if dopt["category"] != "adagrad" else 4, dtype=f32, device=dev)
         self.opt_step = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -470,6 +569,7 @@ class FusedCTR:
         if self.dcn:
             self._cross_init_buffers()
         self._grad_dirty = False
+        self.load_generation = 0     # counts ``load`` calls: rows and plans prefetched before one are stale
         # persistent GEMM chains: forward (fwd1 -> ... -> fwdL) and backward (dX / dW of every layer) in ONE launch
         # each (csrc/cuda/gemm_wgmma.cu: exb_gemm_chain_kernel). EXB_GEMM_CHAIN=0: one launch per GEMM.
         mode = os.environ.get("EXB_GEMM_CHAIN", "bwd")          # "0" | "bwd" | "1" (forward and backward)
@@ -893,6 +993,158 @@ class FusedCTR:
         n += 1 + 5 * self.cross_layers if self.dcn else 0
         return n + (1 if self._ar is not None and not self._rider else 0)
 
+    # ---- dense state, checkpoints and export (all through ``self.layout``)
+    def config(self):
+        """the configuration a checkpoint records; ``CONFIG_KEYS`` must match on load"""
+        return {"model": self.model, "vocab": list(self.vocab), "cached": list(self.cached), "embedding_dim": self.D,
+                "num_dense": self.nd, "hidden": list(self.hidden), "cin_layers": list(self.cin_layers),
+                "cin_split_half": self.cin_split_half if self.cin else None, "cross_layers": self.cross_layers,
+                "pack_linear": self.pack_linear, "batch": self.B, "world": self.ctx.world,
+                "dense_optimizer": self.dense_opt["category"]}
+
+    def config_mismatches(self, config):
+        """one line per configuration entry in which ``config`` differs from this model's"""
+        mine = self.config()
+        return ["%s: checkpoint %r, model %r" % (k, config.get(k), mine[k]) for k in CONFIG_KEYS if config.get(k) != mine[k]]
+
+    def dense_state_dict(self, include_optimizer=True):
+        """The dense parameters as fp32 CPU tensors under ``layout``'s logical names. ``include_optimizer``: plus the
+        dense optimizer's state slots ("<category>.<slot>/<name>", ``DENSE_OPT_SLOTS``) and its step counter
+        ("opt_step"). Reads the buffers after every step launched so far on the current stream."""
+        sd = self.layout.gather(self.theta.cpu())
+        if include_optimizer:
+            cat = self.dense_opt["category"]
+            for slot, buf in zip(DENSE_OPT_SLOTS[cat], (self.accum, self.accum2)):
+                for name, t in self.layout.gather(buf.cpu()).items():
+                    sd["%s.%s/%s" % (cat, slot, name)] = t
+            sd["opt_step"] = self.opt_step.cpu()
+        return sd
+
+    def _dense_buffers(self, sd, config=None):
+        """(theta, accum, accum2, opt_step) on the CPU from a dense state dict: every slot outside the layout at its
+        construction value, the optimizer state fresh unless ``sd`` holds all of this model's dense-optimizer slots.
+        Raises ValueError (nothing changed yet) on a configuration or parameter mismatch."""
+        errs = self.config_mismatches(config) if config is not None else []
+        for name, (shape, _) in self.layout.params.items():
+            t = sd.get(name)
+            if t is None:
+                errs.append("%s: missing" % name)
+            elif tuple(t.shape) != tuple(shape):
+                errs.append("%s: checkpoint shape %s, model %s" % (name, tuple(t.shape), tuple(shape)))
+        if errs:
+            raise ValueError("the checkpoint does not fit this FusedCTR:\n  " + "\n  ".join(errs))
+        f32, n = torch.float32, self.n_theta
+        theta = torch.zeros(n, dtype=f32)
+        self.layout.scatter(theta, sd)
+        accum = torch.full((n,), self._acc0, dtype=f32)
+        accum2 = torch.zeros(self.accum2.numel(), dtype=f32)
+        step = torch.zeros(1, dtype=torch.int32)
+        # a checkpoint without optimizer state, or of another category: the weights load, the state starts fresh
+        # (as the sparse tables do, checkpoint.load_model); the hyper-parameters are always the model's own
+        cat = self.dense_opt["category"]
+        slots = DENSE_OPT_SLOTS[cat]
+        if "opt_step" in sd and all("%s.%s/%s" % (cat, s, p) in sd for s in slots for p in self.layout.params):
+            for s, buf in zip(slots, (accum, accum2)):
+                self.layout.scatter(buf, {p: sd["%s.%s/%s" % (cat, s, p)] for p in self.layout.params})
+            step.copy_(sd["opt_step"].reshape(1))
+        return theta, accum, accum2, step
+
+    def _set_dense(self, bufs):
+        """copy (theta, accum, accum2, opt_step) IN PLACE (captured graphs hold these addresses), clear the
+        gradients, refresh the bf16 weight copies"""
+        for dst, src in zip((self.theta, self.accum, self.accum2, self.opt_step), bufs):
+            dst.copy_(src)
+        self.gtheta.zero_()
+        self._grad_dirty = False
+        self.refresh_weights()
+
+    def load_dense_state_dict(self, sd, config=None):
+        """Load ``dense_state_dict`` output in place (``config``: a checkpoint's ``config()``, checked first). Slots
+        outside the layout (padding) return to their construction values; the gradients are cleared. A different
+        batch size or world size is fine."""
+        self._set_dense(self._dense_buffers(sd, config))
+
+    def save(self, path, include_optimizer=True):
+        """Collective checkpoint into the directory ``path`` (a local path): ``model.pt`` (rank 0, ``torch.save`` of
+        {"format", "config", "dense": dense_state_dict}) and the sparse tables under ``openembedding/`` in the
+        server-model format (``checkpoint.save_model``). Holds the state after every step launched so far; changes
+        nothing, so a prefetched next batch stays valid. The dense state is replicated: every rank holds the same."""
+        ctx = self.ctx
+        torch.cuda.synchronize(self.dev)
+        if ctx.rank == 0:
+            os.makedirs(path, exist_ok=True)
+            torch.save({"format": CHECKPOINT_FORMAT, "config": self.config(),
+                        "dense": self.dense_state_dict(include_optimizer)}, os.path.join(path, "model.pt"))
+            if os.path.exists(os.path.join(path, "openembedding")):
+                shutil.rmtree(os.path.join(path, "openembedding"))
+        ctx.barrier()
+        from .. import checkpoint
+        checkpoint.save_model(ctx, os.path.join(path, "openembedding"), include_optimizer=include_optimizer)
+
+    def load(self, path):
+        """Collective: restore a ``save`` checkpoint -- the tables (rows, hash slots, optimizer states) and the dense
+        state, in place. The configuration must match (ValueError naming each difference, model untouched); batch
+        and world size may differ. A checkpoint without dense-optimizer state, or of another optimizer category,
+        loads the weights and starts that state fresh. Rows or plans prefetched before the load are stale:
+        ``load_generation`` advances and ``FusedTrainer.step`` pulls up front again."""
+        blob = torch.load(os.path.join(path, "model.pt"), map_location="cpu", weights_only=True)
+        if not isinstance(blob, dict) or blob.get("format") != CHECKPOINT_FORMAT:
+            raise ValueError("%s is not a FusedCTR checkpoint" % os.path.join(path, "model.pt"))
+        bufs = self._dense_buffers(blob["dense"], blob["config"])
+        torch.cuda.synchronize(self.dev)
+        from .. import checkpoint
+        checkpoint.load_model(self.ctx, os.path.join(path, "openembedding"))
+        self._set_dense(bufs)
+        self.load_generation += 1
+        torch.cuda.synchronize(self.dev)
+
+    def to_original(self):
+        """The model as a ``models.ctr.StandaloneCTR`` on the CPU: every table row pulled through the engine
+        (collective), the dense weights through ``layout``, ``dnn_out.bias`` folded into ``bias``."""
+        from .ctr import StandaloneCTR
+        if any(self.vocab[f] <= 0 for f in self.server):
+            raise ValueError("can not convert sparse variable to nn.Embedding.")
+        mod = StandaloneCTR(self.vocab, num_dense=self.nd, embedding_dim=self.D, model=self.model, hidden=self.hidden,
+                            cached=self.cached, cin_layers=self.cin_layers or (128, 128),
+                            cin_split_half=self.cin_split_half, cross_layers=self.cross_layers or 3)
+        sd = self.dense_state_dict(include_optimizer=False)
+        sd["bias"] = sd["bias"] + sd.pop("dnn_out.bias")
+        missing, unexpected = mod.load_state_dict(sd, strict=False)
+        assert not unexpected and all(k.startswith(("emb.", "lin.", "cache_cols", "cache_offsets")) for k in missing), \
+            (missing, unexpected)
+        ns, D = self.ns, self.D
+        metas = self.sparse.metas
+        with torch.no_grad():
+            for j, f in enumerate(self.server):
+                if self.pack_linear:
+                    rows = self._pull_table(metas[j], self.vocab[f])
+                    mod.emb[j].weight.copy_(rows[:, :D])
+                    mod.lin[j].weight.copy_(rows[:, D:])
+                else:
+                    mod.emb[j].weight.copy_(self._pull_table(metas[j], self.vocab[f]))
+                    mod.lin[j].weight.copy_(self._pull_table(metas[ns + j], self.vocab[f]))
+        return mod
+
+    def _pull_table(self, meta, vocab):
+        """all rows of a table (CPU fp32 [vocab, dim]), pulled in blocks (collective)"""
+        out = torch.empty(vocab, meta.dim, dtype=torch.float32)
+        blk = 2 ** 20 // meta.dim + 1
+        for i in range(0, vocab, blk):
+            idx = torch.arange(i, min(vocab, i + blk), device=self.dev)
+            out[i:i + idx.numel()] = self.ctx.backend.pull(meta, idx).cpu()
+        return out
+
+    def save_as_original_model(self, path):
+        """Collective export of a stand-alone ``models.ctr.StandaloneCTR`` (fp32, no engine, no GPU) to the file
+        ``path``: every rank pulls, rank 0 writes ``torch.save(module)``. Returns the module (CPU). A hash-table
+        feature (vocab <= 0) cannot become an ``nn.Embedding``: ValueError."""
+        mod = self.to_original()
+        if self.ctx.rank == 0:
+            os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+            torch.save(mod.cpu(), path)
+        self.ctx.barrier()
+        return mod
+
     # ---- fp32 torch reference of the dense math on the current X32 (tests)
     def reference(self, ids, dense, labels, return_logits=False):
         """returns (loss, grads dict) computed with torch autograd in fp32 from the same
@@ -1029,6 +1281,7 @@ class FusedTrainer:
         self.graph = None
         self._ar = model._ar
         self._x32_key = None         # key of the batch whose rows + plan the last step prefetched into X32
+        self._load_gen = model.load_generation     # a model ``load`` since the prefetch makes it stale
         self._warm = False
         self._eval = None            # static eval inputs (ids, dense, labels, n on the device) of predict / evaluate
 
@@ -1040,6 +1293,7 @@ class FusedTrainer:
         inputs into the trainer's own static buffers first (four device copies per step)."""
         g = self.m.group
         v2 = getattr(g, "v2", False)
+        self._drop_stale_prefetch()
         pulled = self._x32_key is not None and self._x32_key == g._key(ids)
         tail = next_ids is not None
         if not self.use_graph:
@@ -1079,6 +1333,16 @@ class FusedTrainer:
         self.graph = gr
         self.ctx.step_done()
         return self._static["loss"]
+
+    def _drop_stale_prefetch(self):
+        """after a ``FusedCTR.load`` the prefetched rows (and, v2, the plan: hash-slot positions) describe tables
+        that are gone: the next step pulls and plans up front"""
+        if self._load_gen == self.m.load_generation:
+            return
+        if self._x32_key is not None and getattr(self.m.group, "v2", False):
+            self.m.group.reset_slot(0)
+        self._x32_key = None
+        self._load_gen = self.m.load_generation
 
     def _capture(self, key, s):
         head, tail = key[:2]

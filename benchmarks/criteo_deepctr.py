@@ -24,7 +24,7 @@ from openembedding_b200.models.ctr import CRITEO_1TB_VOCAB_20M, CRITEO_KAGGLE_VO
 from openembedding_b200.models.trainer import Trainer  # noqa: E402
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--model", default="DeepFM", help="LR|WDL|DeepFM|xDeepFM|DCN|all")
+ap.add_argument("--model", default="DeepFM", help="LR|WDL|DeepFM|xDeepFM|DCN|AutoInt|all")
 ap.add_argument("--embedding_dim", default="64", help="comma list, e.g. 9,64")
 ap.add_argument("--optimizer", default="adagrad")
 ap.add_argument("--batch_size", type=int, default=4096)
@@ -36,7 +36,7 @@ ap.add_argument("--steps", type=int, default=100)
 ap.add_argument("--warmup", type=int, default=10)
 ap.add_argument("--cpu", action="store_true")
 ap.add_argument("--engine", default="auto", choices=["auto", "fused", "eager"],
-                help="fused: FusedCTR + FusedTrainer (WDL / DeepFM / xDeepFM / DCN, CUDA); eager: CTRModel + Trainer; "
+                help="fused: FusedCTR + FusedTrainer (WDL / DeepFM / xDeepFM / DCN / AutoInt, CUDA); eager: CTRModel + Trainer; "
                      "auto: fused where it exists")
 ap.add_argument("--profile", default="", help="directory: write a chrome trace of 10 steps after the timed run "
                                                 "(reference: --profile / TensorBoard profile_batch, criteo_deepctr.py:290-293), "
@@ -53,16 +53,16 @@ oe.flags.device = "cuda" if use_cuda else "cpu"
 vocab = CRITEO_KAGGLE_VOCAB if a.vocab == "kaggle" else CRITEO_1TB_VOCAB_20M
 if a.cpu:
     vocab = [min(v, 100000) for v in vocab]
-models = ["LR", "WDL", "DeepFM", "xDeepFM", "DCN"] if a.model == "all" else [a.model]
+models = ["LR", "WDL", "DeepFM", "xDeepFM", "DCN", "AutoInt"] if a.model == "all" else [a.model]
 for name in models:
     for dim in (int(x) for x in a.embedding_dim.split(",")):
         reset_context()
         ctx = get_context()
         dev = ctx.device
-        can_fuse = use_cuda and name.lower() in ("deepfm", "wdl", "xdeepfm", "dcn") and a.batch_size % 128 == 0
+        can_fuse = use_cuda and name.lower() in ("deepfm", "wdl", "xdeepfm", "dcn", "autoint") and a.batch_size % 128 == 0
         if a.engine == "fused" and not can_fuse:
-            raise SystemExit("--engine fused: %s at batch %d has no fused step (CUDA, WDL / DeepFM / xDeepFM / DCN, "
-                             "batch %% 128 == 0)" % (name, a.batch_size))
+            raise SystemExit("--engine fused: %s at batch %d has no fused step (CUDA, WDL / DeepFM / xDeepFM / DCN / "
+                             "AutoInt, batch %% 128 == 0)" % (name, a.batch_size))
         fused = can_fuse and a.engine != "eager"
         cache = a.batch_size if a.cache else 0
         if fused:

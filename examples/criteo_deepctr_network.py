@@ -1,4 +1,4 @@
-"""DeepFM / WDL / xDeepFM / DCN on Criteo-shaped data -- counterpart of the reference's
+"""DeepFM / WDL / xDeepFM / DCN / AutoInt on Criteo-shaped data -- counterpart of the reference's
 examples/criteo_deepctr_network{,_mirrored,_mpi}.py and test/benchmark/criteo_deepctr.py.
 
 single GPU / CPU :  python examples/criteo_deepctr_network.py --model DeepFM
@@ -24,13 +24,13 @@ from openembedding_b200.models.trainer import Trainer  # noqa: E402
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--data", default="")
-ap.add_argument("--model", default="DeepFM", choices=["LR", "WDL", "DeepFM", "xDeepFM", "DCN"])
+ap.add_argument("--model", default="DeepFM", choices=["LR", "WDL", "DeepFM", "xDeepFM", "DCN", "AutoInt"])
 ap.add_argument("--optimizer", default="Adagrad", choices=["Adam", "Adagrad", "Ftrl", "SGD"])
 ap.add_argument("--embedding_dim", type=int, default=9)
 ap.add_argument("--batch_size", type=int, default=16)
 ap.add_argument("--epochs", type=int, default=3)
 ap.add_argument("--cache", action="store_true", help="replicate tables smaller than the batch (sparse_as_dense)")
-ap.add_argument("--fused", action="store_true", help="whole step on the hand-written kernels (CUDA, DeepFM/WDL/xDeepFM/DCN)")
+ap.add_argument("--fused", action="store_true", help="whole step on the hand-written kernels (CUDA, DeepFM/WDL/xDeepFM/DCN/AutoInt)")
 ap.add_argument("--validation_batches", type=int, default=0,
                 help="with --fused: hold out the last N batches of each rank, print val_auc / val_logloss per epoch")
 ap.add_argument("--cpu", action="store_true")
@@ -74,8 +74,8 @@ n_train = n - n_val
 sparse_opt = {"category": args.optimizer.lower()}
 cache = args.batch_size if args.cache else 0
 if args.fused:
-    if args.model not in ("WDL", "DeepFM", "xDeepFM", "DCN"):
-        raise SystemExit("--fused: WDL, DeepFM, xDeepFM or DCN")
+    if args.model not in ("WDL", "DeepFM", "xDeepFM", "DCN", "AutoInt"):
+        raise SystemExit("--fused: WDL, DeepFM, xDeepFM, DCN or AutoInt")
     from openembedding_b200.models.fused_dense import FusedCTR, FusedTrainer
     model = FusedCTR(vocab, embedding_dim=args.embedding_dim, model=args.model.lower(), batch=args.batch_size,
                      sparse_optimizer=sparse_opt, cache_threshold=cache)

@@ -1,4 +1,4 @@
-"""CTR model zoo on the sharded engine: LR, Wide&Deep, DeepFM, xDeepFM, DCN-v2.
+"""CTR model zoo on the sharded engine: LR, Wide&Deep, DeepFM, xDeepFM, DCN-v2, AutoInt.
 
 The reference benchmarks DeepCTR's WDL / DeepFM / xDeepFM with every
 ``keras.layers.Embedding`` swapped for the PS embedding
@@ -181,12 +181,62 @@ class CrossNetV2(nn.Module):
         return x
 
 
+class InteractingLayer(nn.Module):
+    """AutoInt's multi-head self-attention over the fields (DeepCTR ``InteractingLayer``, ``scaling=False``) in fp32
+    torch: x [B, nf, in_dim] -> relu(concat_heads(softmax(Q K^T) V) + x W_res) [B, nf, d * heads], with
+    Q = x W_query, K = x W_key, V = x W_value; head h owns the columns h*d .. h*d + d - 1. Weights [in_dim, d * heads],
+    no bias, Keras TruncatedNormal(stddev 0.05) initial values."""
+
+    def __init__(self, in_dim, att_embedding_size=8, head_num=2, use_res=True):
+        super().__init__()
+        self.d, self.heads, self.use_res = att_embedding_size, head_num, use_res
+        names = ("W_query", "W_key", "W_value") + (("W_res",) if use_res else ())
+        for n in names:
+            w = nn.Parameter(torch.empty(in_dim, att_embedding_size * head_num))
+            nn.init.trunc_normal_(w, std=0.05, a=-0.1, b=0.1)
+            setattr(self, n, w)
+
+    @staticmethod
+    def attend(q, k, v, r, heads):
+        """relu(concat_heads(softmax(q_h k_h^T) v_h) + r) from the projections q, k, v [B, nf, d * heads] and r (the
+        residual projection, or None)"""
+        B, nf, dh = q.shape
+        split = lambda t: t.view(B, nf, heads, dh // heads).transpose(1, 2)       # [B, heads, nf, d]
+        p = torch.softmax(split(q) @ split(k).transpose(-1, -2), dim=-1)
+        o = (p @ split(v)).transpose(1, 2).reshape(B, nf, dh)
+        return F.relu(o + r if r is not None else o)
+
+    def forward(self, x):
+        r = x @ self.W_res if self.use_res else None
+        return self.attend(x @ self.W_query, x @ self.W_key, x @ self.W_value, r, self.heads)
+
+
+class AutoIntNet(nn.Module):
+    """``layers`` stacked ``InteractingLayer``s: the first takes the embedding dim, the others d * heads"""
+
+    def __init__(self, embedding_dim, layers=3, att_embedding_size=8, head_num=2, use_res=True):
+        super().__init__()
+        dims = [embedding_dim] + [att_embedding_size * head_num] * layers
+        self.layers = nn.ModuleList([InteractingLayer(dims[l], att_embedding_size, head_num, use_res)
+                                     for l in range(layers)])
+        self.out_dim = att_embedding_size * head_num
+
+    def forward(self, x):
+        for layer in self.layers:
+            x = layer(x)
+        return x
+
+
+AUTOINT_DEFAULTS = dict(att_layers=3, att_embedding_size=8, att_head_num=2, att_res=True)
+
+
 class _CTRHead(nn.Module):
     """The dense part of the zoo's CTR models, shared by ``CTRModel`` and ``StandaloneCTR``: the layers after the
     row lookup, and the logit from the looked-up rows."""
 
-    def _build_dense(self, num_dense, dnn_hidden, tc, cin_layers, cross_layers, cin_split_half=True):
-        """dense_linear, bias and (models with embeddings) dnn, dnn_out, cin / cin_out, cross"""
+    def _build_dense(self, num_dense, dnn_hidden, tc, cin_layers, cross_layers, cin_split_half=True, autoint=None):
+        """dense_linear, bias and (models with embeddings) dnn, dnn_out, cin / cin_out, cross, att (``autoint``:
+        ``AUTOINT_DEFAULTS``' keys)"""
         nf, embedding_dim = self.nf, self.D
         dnn_in = nf * embedding_dim + num_dense
         self.tc = tc
@@ -206,6 +256,11 @@ class _CTRHead(nn.Module):
         if self.model_name == "dcn":
             self.cross = CrossNetV2(dnn_in, cross_layers, tc=tc)
             self.dnn_out = nn.Linear(prev + dnn_in, 1, bias=False)
+        if self.model_name == "autoint":        # DeepCTR's concat order: flatten(attention output), then the DNN
+            a = dict(AUTOINT_DEFAULTS, **(autoint or {}))
+            self.att = AutoIntNet(embedding_dim, a["att_layers"], a["att_embedding_size"], a["att_head_num"],
+                                  a["att_res"])
+            self.dnn_out = nn.Linear(nf * self.att.out_dim + prev, 1, bias=False)
 
     def _cached_rows(self, ids, embs, lins):
         """append the rows of the replicated ("cache") tables to the embedding / linear parts"""
@@ -232,6 +287,11 @@ class _CTRHead(nn.Module):
             if self.model_name == "dcn":
                 h = torch.cat([self.cross(x), self.dnn(x)], dim=1)
                 logit = logit + self.dnn_out(h).squeeze(-1).float()
+            elif self.model_name == "autoint":
+                with torch.autocast(device_type=emb.device.type, enabled=False):      # the attention runs in fp32
+                    att = self.att(emb).reshape(B, -1)
+                h = torch.cat([att, self.dnn(x)], dim=1)
+                logit = logit + self.dnn_out(h).squeeze(-1).float()
             else:
                 logit = logit + self.dnn_out(self.dnn(x)).squeeze(-1).float()
             if self.model_name == "xdeepfm":
@@ -242,12 +302,18 @@ class _CTRHead(nn.Module):
         return logit
 
 
+def _default_hidden(model):
+    """DeepCTR's default DNN of each model"""
+    return {"wdl": (512, 256, 128, 32), "autoint": (256, 128, 64)}.get(model, (400, 400, 400))
+
+
 class CTRModel(_CTRHead):
-    """model in {"lr", "wdl", "deepfm", "xdeepfm", "dcn"}"""
+    """model in {"lr", "wdl", "deepfm", "xdeepfm", "dcn", "autoint"}"""
 
     def __init__(self, vocab_sizes, num_dense=13, embedding_dim=9, model="deepfm", batch=4096,
                  sparse_optimizer=None, dnn_hidden=None, cache_threshold=0, num_shards=None,
-                 compute_dtype=torch.bfloat16, cin_layers=(128, 128), cross_layers=3):
+                 compute_dtype=torch.bfloat16, cin_layers=(128, 128), cross_layers=3, att_layers=3, att_embedding_size=8,
+                 att_head_num=2, att_res=True):
         super().__init__()
         ctx = get_context()
         self.model_name = model.lower()
@@ -257,7 +323,7 @@ class CTRModel(_CTRHead):
         nf = len(vocab_sizes)
         self.nf = nf
         if dnn_hidden is None:
-            dnn_hidden = (512, 256, 128, 32) if self.model_name == "wdl" else (400, 400, 400)
+            dnn_hidden = _default_hidden(self.model_name)
         if sparse_optimizer is None:
             sparse_optimizer = {"category": "adagrad"}   # tf.keras.optimizers.Adagrad() defaults
         zero = {"category": "constant", "value": 0.0}    # benchmark uses zeros initializer (criteo_deepctr.py:82)
@@ -289,7 +355,9 @@ class CTRModel(_CTRHead):
             self.cache_lin = nn.Parameter(torch.zeros(off, 1, device=ctx.device))
         # GEMM-shaped layers on the hand-written wgmma kernel (bf16 operands) when the model computes in bf16 on CUDA
         tc = ctx.device.type == "cuda" and compute_dtype == torch.bfloat16
-        self._build_dense(num_dense, dnn_hidden, tc, cin_layers, cross_layers)
+        self._build_dense(num_dense, dnn_hidden, tc, cin_layers, cross_layers,
+                          autoint=dict(att_layers=att_layers, att_embedding_size=att_embedding_size,
+                                       att_head_num=att_head_num, att_res=att_res))
         self.to(ctx.device)
 
     def dense_parameters(self):
@@ -314,24 +382,25 @@ class CTRModel(_CTRHead):
 
 
 class StandaloneCTR(_CTRHead):
-    """A trained Wide&Deep / DeepFM / xDeepFM / DCN-v2 as a plain fp32 module that needs no engine and no GPU (the
+    """A trained Wide&Deep / DeepFM / xDeepFM / DCN-v2 / AutoInt as a plain fp32 module that needs no engine and no GPU (the
     export of ``FusedCTR.save_as_original_model``): ``emb[j]`` (dim D) and ``lin[j]`` (dim 1) are the
     ``nn.Embedding`` tables of the j-th server feature, ``cache_emb`` / ``cache_lin`` the replicated tables of the
     ``cached`` features, and the dense layers carry ``CTRModel``'s names. ``forward(ids [B, nf], dense [B, nd])``
     returns fp32 logits [B]."""
 
     def __init__(self, vocab_sizes, num_dense=13, embedding_dim=9, model="deepfm", hidden=None, cached=(),
-                 cin_layers=(128, 128), cin_split_half=True, cross_layers=3):
+                 cin_layers=(128, 128), cin_split_half=True, cross_layers=3, att_layers=3, att_embedding_size=8,
+                 att_head_num=2, att_res=True):
         super().__init__()
         self.model_name = model.lower()
-        if self.model_name not in ("wdl", "deepfm", "xdeepfm", "dcn"):
-            raise ValueError("StandaloneCTR: wdl, deepfm, xdeepfm or dcn")
+        if self.model_name not in ("wdl", "deepfm", "xdeepfm", "dcn", "autoint"):
+            raise ValueError("StandaloneCTR: wdl, deepfm, xdeepfm, dcn or autoint")
         self.num_dense, self.D = num_dense, embedding_dim
         self.vocab_sizes = list(vocab_sizes)
         self.nf = nf = len(self.vocab_sizes)
         self.compute_dtype, self.has_emb = torch.float32, True
         if hidden is None:
-            hidden = (512, 256, 128, 32) if self.model_name == "wdl" else (400, 400, 400)
+            hidden = _default_hidden(self.model_name)
         self.cached = list(cached)
         self.server = [f for f in range(nf) if f not in self.cached]
         self.emb = nn.ModuleList([nn.Embedding(self.vocab_sizes[f], embedding_dim) for f in self.server])
@@ -343,7 +412,9 @@ class StandaloneCTR(_CTRHead):
             self.register_buffer("cache_cols", torch.tensor(self.cached, dtype=torch.int64))
             self.cache_emb = nn.Parameter(torch.zeros(rows, embedding_dim))
             self.cache_lin = nn.Parameter(torch.zeros(rows, 1))
-        self._build_dense(num_dense, hidden, False, cin_layers, cross_layers, cin_split_half)
+        self._build_dense(num_dense, hidden, False, cin_layers, cross_layers, cin_split_half,
+                          autoint=dict(att_layers=att_layers, att_embedding_size=att_embedding_size,
+                                       att_head_num=att_head_num, att_res=att_res))
 
     def forward(self, ids, dense):
         embs, lins = [], []

@@ -1,4 +1,4 @@
-"""Fused DeepFM / Wide&Deep / xDeepFM / DCN-v2 training step on hand-written sm_90a kernels only.
+"""Fused DeepFM / Wide&Deep / xDeepFM / DCN-v2 / AutoInt training step on hand-written sm_90a kernels only.
 
 Per step and per GPU (10 launches at world 1, captured in one CUDA graph by ``FusedTrainer``):
 
@@ -26,6 +26,11 @@ interaction backward, filter-gradient GEMM) and the fold of the CIN embedding gr
 DCN-v2 adds the cross network on the A0 layout (csrc/cuda/cross_kernels.cu + the wgmma GEMM), 1 + 5 L launches for
 L layers: L x (U_l GEMM, cross forward) before the head; after the dX GEMM, the top of the cross backward and
 L x (P_l GEMM, weight-gradient GEMM, cross backward), the last of which folds the embedding gradient into G32.
+
+AutoInt adds stacked multi-head self-attention over the fields (csrc/cuda/autoint_kernels.cu + the wgmma GEMM) on rows
+r = (sample, field), 2 + 5 A launches for A layers: gather + A x (projection GEMM, attention forward) before the head;
+after the dX GEMM, A x (attention backward, weight-gradient GEMM, input-gradient GEMM) and the fold of the embedding
+gradient (and of the partial sums of the output weight's gradient) into G32 / gtheta.
 
 Evaluation (``predict_forward``; ``FusedTrainer.predict`` / ``evaluate``) runs the forward half alone: stateless pull,
 prep, the forward GEMMs, the CIN / cross forward and the predict head (logits + probabilities, dense_kernels.cu).
@@ -115,6 +120,18 @@ class _CrossBwdArgs(ctypes.Structure):
                 ("XfL", c_void_p), ("g_wcross", c_void_p), ("main_ctas", c_int)]
 
 
+class _AttFwdArgs(ctypes.Structure):
+    _fields_ = [("QKVR", c_void_p), ("Np", c_int), ("P", c_void_p), ("Xf", c_void_p), ("Xb", c_void_p), ("ldxb", c_int),
+                ("watt", c_void_p), ("base", c_void_p), ("B", c_int), ("nf", c_int), ("d", c_int), ("h", c_int),
+                ("res", c_int)]
+
+
+class _AttBwdArgs(ctypes.Structure):
+    _fields_ = [("QKVR", c_void_p), ("Np", c_int), ("P", c_void_p), ("Xf", c_void_p), ("dX", c_void_p), ("lddx", c_int),
+                ("dlogit", c_void_p), ("watt", c_void_p), ("dQKVR", c_void_p), ("gpart", c_void_p), ("B", c_int),
+                ("nf", c_int), ("d", c_int), ("h", c_int), ("res", c_int), ("main_ctas", c_int)]
+
+
 def _r(x, m):
     return (x + m - 1) // m * m
 
@@ -196,6 +213,60 @@ def _cross_ck(rc, what):
         raise RuntimeError("%s: %s" % (what, _cross_lib().exb_cross_last_error().decode()))
 
 
+_att_proto = False
+
+
+def _att_lib():
+    global _att_proto
+    lib = _native.cuda()
+    if not _att_proto:
+        u64 = ctypes.c_uint64
+        for fn in (lib.exb_att_fwd, lib.exb_att_bwd):
+            fn.restype = c_int
+            fn.argtypes = [c_void_p, u64]
+        lib.exb_att_gather.restype = c_int
+        lib.exb_att_gather.argtypes = [u64, c_longlong, c_int, c_int, c_int, u64, c_int, c_int, u64]
+        lib.exb_att_fold.restype = c_int
+        lib.exb_att_fold.argtypes = [u64, c_longlong, c_int, c_int, c_int, u64, c_int, c_int, u64, c_int, u64, u64]
+        lib.exb_att_last_error.restype = ctypes.c_char_p
+        assert lib.exb_att_fwd_args_size() == ctypes.sizeof(_AttFwdArgs), "AttFwdArgs ABI mismatch"
+        assert lib.exb_att_bwd_args_size() == ctypes.sizeof(_AttBwdArgs), "AttBwdArgs ABI mismatch"
+        _att_proto = True
+    return lib
+
+
+def _att_ck(rc, what):
+    if rc != 0:
+        raise RuntimeError("%s: %s" % (what, _att_lib().exb_att_last_error().decode()))
+
+
+AUTOINT_MAX_FIELDS = 64    # csrc/cuda/autoint_kernels.cu: two attention scores per lane of a warp
+AUTOINT_MAX_WIDTH = 64     # d * heads: X_{l+1}'s bf16 operand is one 64-column K block of the next projection
+
+
+def autoint_dims(nf, layers, d, h, res, embedding_dim=1, dnn_layers=0):
+    """Sizes of the fused AutoInt: (dh, Np, Kp). dh = d * h is a layer's output width, Np = r(4 dh, 64)
+    (r(3 dh, 64) without the residual) the width of the stacked projection [Q | K | V | R], Kp[l] the padded input
+    width of layer l: r(embedding_dim, 64), then r(dh, 64) = 64. Raises ValueError for the sizes the kernels and the
+    dense optimizer do not take: no layer, nf outside 1 .. 64, d or h below 1, d * h above 64, or more than 8 weight
+    matrices with the ``dnn_layers`` of the DNN."""
+    layers, d, h = int(layers), int(d), int(h)
+    if layers < 1:
+        raise ValueError("AutoInt needs at least one attention layer (got %d)" % layers)
+    if not 1 <= nf <= AUTOINT_MAX_FIELDS:
+        raise ValueError("the attention kernels take 1 .. %d fields (got %d)" % (AUTOINT_MAX_FIELDS, nf))
+    if d < 1 or h < 1:
+        raise ValueError("att_embedding_size and att_head_num must be positive (got %d, %d)" % (d, h))
+    if d * h > AUTOINT_MAX_WIDTH:
+        raise ValueError("att_embedding_size * att_head_num = %d is above %d" % (d * h, AUTOINT_MAX_WIDTH))
+    if dnn_layers + layers > _OPT_MAX_MATS:
+        raise ValueError("the fused optimizer kernel takes at most %d weight matrices (DNN + attention layers)"
+                         % _OPT_MAX_MATS)
+    dh = d * h
+    Np = _r((4 if res else 3) * dh, 64)
+    return dh, Np, [_r(int(embedding_dim), 64)] + [_r(dh, 64)] * (layers - 1)
+
+
 def cross_cols(nf, D, Dp, nd):
     """Columns of the A0 layout [nf*Dp embedding | nd dense | pad | ones] that hold DCN-v2's input
     x = [emb (nf*D) | dense (nd)], in the order of x: field j's embedding column d < D is column j*Dp + d, the
@@ -275,7 +346,7 @@ class DenseLayout:
 
 
 def dense_layout(vocab_sizes, num_dense, embedding_dim, model, hidden, cached=(), cin_layers=(128, 128),
-                 cin_split_half=True, cross_layers=3):
+                 cin_split_half=True, cross_layers=3, att_layers=3, att_embedding_size=8, att_head_num=2, att_res=True):
     """The ``DenseLayout`` of a ``FusedCTR`` configuration (``cached``: the features held in the replicated table).
     Needs no GPU: save, load and export read and write the dense state through this map alone."""
     vocab, model, hidden = list(vocab_sizes), model.lower(), [int(h) for h in hidden]
@@ -300,6 +371,11 @@ def dense_layout(vocab_sizes, num_dense, embedding_dim, model, hidden, cached=()
     Lc = int(cross_layers) if model == "dcn" else 0
     for l in range(Lc):                 # bias in the ones column K0p - 1
         seg("X%d" % l, K0p, K0p)
+    La = int(att_layers) if model == "autoint" else 0
+    if La:                              # [W_query | W_key | W_value | W_res] of layer l, [in, out] as in DeepCTR
+        adh, aNp, aKp = autoint_dims(nf, La, att_embedding_size, att_head_num, att_res, D, len(hidden))
+        for l in range(La):
+            seg("T%d" % l, aKp[l], aNp)
     seg("wout", 1, Hp[-1])
     seg("wd", 1, max(nd, 1))
     seg("bias", 1, 1)
@@ -308,6 +384,8 @@ def dense_layout(vocab_sizes, num_dense, embedding_dim, model, hidden, cached=()
         seg("wcin", 1, T)
     if Lc:
         seg("wcross", 1, K0p)
+    if La:
+        seg("watt", 1, nf * adh)
     vc = sum(vocab[f] for f in cached)
     seg("cache_emb", vc, Dp)
     seg("cache_lin", 1, vc, n=max(vc, 1))
@@ -321,6 +399,8 @@ def dense_layout(vocab_sizes, num_dense, embedding_dim, model, hidden, cached=()
     hL = hidden[-1]
     if Lc:                              # CTRModel's order: cat([cross(x), dnn(x)])
         params["dnn_out.weight"] = ((1, len(real0) + hL), [("wcross", [0], real0), ("wout", [0], range(hL))])
+    elif La:                            # CTRModel's order: cat([flatten(att(emb)), dnn(x)])
+        params["dnn_out.weight"] = ((1, nf * adh + hL), [("watt", [0], range(nf * adh)), ("wout", [0], range(hL))])
     else:
         params["dnn_out.weight"] = ((1, hL), [("wout", [0], range(hL))])
     params["dnn_out.bias"] = ((1,), [("wout", [0], [Hp[-1] - 1])])
@@ -340,6 +420,11 @@ def dense_layout(vocab_sizes, num_dense, embedding_dim, model, hidden, cached=()
         n = len(real0)
         params["cross.w.%d.weight" % l] = ((n, n), [("X%d" % l, real0, real0)])
         params["cross.w.%d.bias" % l] = ((n,), [("X%d" % l, real0, [K0p - 1])])
+    names = ("W_query", "W_key", "W_value") + (("W_res",) if att_res else ())
+    for l in range(La):
+        d_in = D if l == 0 else adh
+        for k, name in enumerate(names):
+            params["att.layers.%d.%s" % (l, name)] = ((d_in, adh), [("T%d" % l, range(d_in), range(k * adh, (k + 1) * adh))])
     return DenseLayout(segs, off, shapes, params)
 
 
@@ -348,32 +433,33 @@ DENSE_OPT_SLOTS = {"adagrad": ("accumulator",), "adam": ("m", "v"), "ftrl": ("ac
 CHECKPOINT_FORMAT = "openembedding_b200.FusedCTR/1"
 # what a checkpoint must agree on with the model that loads it (batch, world size and optimizer may differ)
 CONFIG_KEYS = ("model", "vocab", "cached", "embedding_dim", "num_dense", "hidden", "cin_layers", "cin_split_half",
-               "cross_layers", "pack_linear")
+               "cross_layers", "pack_linear", "att_layers", "att_embedding_size", "att_head_num", "att_res")
 
 
 class FusedCTR:
-    """DeepFM (use_fm=True), Wide&Deep, xDeepFM or DCN-v2 (use_fm=False; xDeepFM adds the CIN branch, DCN-v2 the
-    cross network) with the whole step on own kernels."""
+    """DeepFM (use_fm=True), Wide&Deep, xDeepFM, DCN-v2 or AutoInt (use_fm=False; xDeepFM adds the CIN branch, DCN-v2
+    the cross network, AutoInt the field self-attention) with the whole step on own kernels."""
 
     def __init__(self, vocab_sizes, num_dense=13, embedding_dim=64, model="deepfm", batch=4096, hidden=None,
                  sparse_optimizer=None, cache_threshold=0, lr=0.001, initial_accumulator_value=0.1, eps=1e-7,
                  num_shards=None, dw_splits=8, seed=0, pack_linear=None, dense_optimizer=None,
-                 cin_layers=(128, 128), cin_split_half=True, cross_layers=3):
-        from .ctr import FusedEmbeddings
+                 cin_layers=(128, 128), cin_split_half=True, cross_layers=3, att_layers=3, att_embedding_size=8,
+                 att_head_num=2, att_res=True):
+        from .ctr import FusedEmbeddings, _default_hidden
         ctx = get_context()
         if ctx.device.type != "cuda":
             raise RuntimeError("FusedCTR runs on the CUDA engine only (use models.ctr.CTRModel on CPU)")
         assert batch % 128 == 0, "the fused dense path needs batch % 128 == 0"
         self.ctx, self.dev, self.lib = ctx, ctx.device, _lib()
         self.model = model.lower()
-        assert self.model in ("deepfm", "wdl", "xdeepfm", "dcn")
+        assert self.model in ("deepfm", "wdl", "xdeepfm", "dcn", "autoint")
         self.use_fm = self.model == "deepfm"
         self.B, self.nd, self.D = batch, num_dense, embedding_dim
         self.Dp = _r(embedding_dim, 4)
         self.vocab = list(vocab_sizes)
         self.nf = len(self.vocab)
         if hidden is None:
-            hidden = (512, 256, 128, 32) if self.model == "wdl" else (400, 400, 400)
+            hidden = _default_hidden(self.model)
         self.hidden = list(hidden)
         # xDeepFM: Compressed Interaction Network over the nf embeddings, rows r = (sample, embedding column)
         self.cin = self.model == "xdeepfm"
@@ -394,6 +480,13 @@ class FusedCTR:
             if len(self.hidden) + self.cross_layers > _OPT_MAX_MATS:
                 raise ValueError("the fused optimizer kernel takes at most %d weight matrices (DNN + cross layers)"
                                  % _OPT_MAX_MATS)
+        # AutoInt: stacked self-attention over the fields, rows r = (sample, field), one stacked projection per layer
+        self.autoint = self.model == "autoint"
+        self.att_layers = int(att_layers) if self.autoint else 0
+        if self.autoint:
+            self.att_d, self.att_h, self.att_res = int(att_embedding_size), int(att_head_num), bool(att_res)
+            self.att_dh, self.att_Np, self.att_Kp = autoint_dims(self.nf, self.att_layers, self.att_d, self.att_h,
+                                                                 self.att_res, embedding_dim, len(self.hidden))
         self.Hp = [_r(h + 1, 64) for h in self.hidden]
         self.lr, self.eps, self.dw_splits = lr, eps, int(os.environ.get("EXB_DW_SPLITS", dw_splits))
         self.cached = [f for f, v in enumerate(self.vocab) if 0 < v < cache_threshold]
@@ -431,12 +524,14 @@ class FusedCTR:
         # by the optimizer), then wout, wd, bias, wcin, wcross (x_L's output weights, zero outside the real columns),
         # cache_emb, cache_lin (dense_layout)
         self.layout = dense_layout(self.vocab, num_dense, embedding_dim, self.model, self.hidden, self.cached,
-                                   self.cin_layers, self.cin_split_half, self.cross_layers)
+                                   self.cin_layers, self.cin_split_half, self.cross_layers, self.att_layers,
+                                   *((self.att_d, self.att_h, self.att_res) if self.autoint else ()))
         segs, off = self.layout.segs, self.layout.n_theta
         dims = [self.K0p] + self.Hp
         L = len(self.hidden)
         K = len(self.cin_layers)
         Lc = self.cross_layers
+        La = self.att_layers
         if self.cin:
             self.cin_T = sum(n - lo for n, lo in zip(self.cin_layers, self.cin_lo))    # pooled CIN features
         self.cache_rows = sum(self.vocab[f] for f in self.cached)
@@ -497,6 +592,17 @@ class FusedCTR:
             for l in range(Lc):
                 blk = torch.randn(n, n, generator=gen) * math.sqrt(2.0 / (n + n))
                 self.xview(l)[self.cross_real[:, None], self.cross_real[None, :]] = blk.to(dev)
+        if self.autoint:            # DeepCTR InteractingLayer: TruncatedNormal(stddev 0.05); w_att, wout one Dense(1)
+            dh, T = self.att_dh, nf * self.att_dh
+            std = math.sqrt(2.0 / (self.hidden[-1] + T + 1))
+            self.view("wout")[: self.hidden[-1]] = (torch.randn(self.hidden[-1], generator=gen) * std).to(dev)
+            self.view("watt")[:] = (torch.randn(T, generator=gen) * std).to(dev)
+            nmat = 4 if self.att_res else 3
+            for l in range(La):
+                d_in = embedding_dim if l == 0 else dh
+                w = torch.empty(d_in, nmat * dh)
+                torch.nn.init.trunc_normal_(w, std=0.05, a=-0.1, b=0.1, generator=gen)
+                self.aview(l)[:d_in, :nmat * dh] = w.to(dev)
         for k in range(K):          # DeepCTR CIN: glorot-uniform filters (fan_in H_k * nf, fan_out N_k), zero biases
             C, n = self.cin_H[k] * nf, self.cin_layers[k]
             lim = math.sqrt(6.0 / (C + n))
@@ -510,6 +616,8 @@ class FusedCTR:
         self.cWTb = [torch.zeros(self.cin_Kp[k], self.cin_Np[k], dtype=bf16, device=dev) for k in range(K)]
         self.xWb = [torch.zeros(self.K0p, self.K0p, dtype=bf16, device=dev) for l in range(Lc)]
         self.xWTb = [torch.zeros(self.K0p, self.K0p, dtype=bf16, device=dev) for l in range(Lc)]
+        self.aWb = [torch.zeros(self.att_Kp[l], self.att_Np, dtype=bf16, device=dev) for l in range(La)]
+        self.aWTb = [torch.zeros(self.att_Np, self.att_Kp[l], dtype=bf16, device=dev) for l in range(La)]
         # ---- activations
         B = batch
         self.X32 = torch.zeros(B, self.XS, dtype=f32, device=dev)
@@ -541,11 +649,11 @@ class FusedCTR:
         self.mn_major = os.environ.get("EXB_MN_MAJOR", "1") != "0"
         self._s2 = torch.cuda.Stream(device=dev)
         self._ev_fork, self._ev_join, self._ev_plan = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
-        assert L + K + Lc <= _OPT_MAX_MATS, "the fused optimizer kernel takes at most %d weight matrices" % _OPT_MAX_MATS
+        assert L + K + Lc + La <= _OPT_MAX_MATS, "the fused optimizer kernel takes at most %d weight matrices" % _OPT_MAX_MATS
         oa = _DenseOptArgs()
         oa.theta, oa.accum, oa.grad = self.theta.data_ptr(), self.accum.data_ptr(), self.gtheta.data_ptr()
         oa.n, oa.flat_lo, oa.lr, oa.eps = self.n_theta, segs["wout"][0], self.lr, float(self.dense_opt.get("epsilon", self.eps))
-        oa.nmat, oa.zero_grad = L + K + Lc, 1
+        oa.nmat, oa.zero_grad = L + K + Lc + La, 1
         d = self.dense_opt
         oa.kind = {"adagrad": 0, "adam": 1, "ftrl": 2}[d["category"]]
         oa.accum2, oa.step = self.accum2.data_ptr(), self.opt_step.data_ptr()
@@ -563,11 +671,17 @@ class FusedCTR:
             i = L + K + l
             oa.mat[i].off, oa.mat[i].R, oa.mat[i].C = segs["X%d" % l][0], self.K0p, self.K0p
             oa.mat[i].Wb, oa.mat[i].WTb = self.xWb[l].data_ptr(), self.xWTb[l].data_ptr()
+        for l in range(La):
+            i = L + K + Lc + l
+            oa.mat[i].off, oa.mat[i].R, oa.mat[i].C = segs["T%d" % l][0], self.att_Kp[l], self.att_Np
+            oa.mat[i].Wb, oa.mat[i].WTb = self.aWb[l].data_ptr(), self.aWTb[l].data_ptr()
         self._opt_args = oa
         if self.cin:
             self._cin_init_buffers()
         if self.dcn:
             self._cross_init_buffers()
+        if self.autoint:
+            self._att_init_buffers()
         self._grad_dirty = False
         self.load_generation = 0     # counts ``load`` calls: rows and plans prefetched before one are stale
         # persistent GEMM chains: forward (fwd1 -> ... -> fwdL) and backward (dX / dW of every layer) in ONE launch
@@ -617,6 +731,11 @@ class FusedCTR:
     def xview(self, l, grad=False):
         """cross layer l's matrix [K0p, K0p] (out, in; bias in the ones column K0p - 1) in theta, or in gtheta"""
         return (self.gview if grad else self.view)("X%d" % l).view(self.K0p, self.K0p)
+
+    def aview(self, l, grad=False):
+        """AutoInt layer l's stacked projection [Kp_l, Np] = [W_query | W_key | W_value | W_res] (in, out) in theta, or
+        in gtheta"""
+        return (self.gview if grad else self.view)("T%d" % l).view(self.att_Kp[l], self.att_Np)
 
     # ---- xDeepFM: the CIN branch (csrc/cuda/cin_kernels.cu + the wgmma GEMM), every buffer allocated here once
     def _cin_init_buffers(self):
@@ -764,6 +883,61 @@ class FusedCTR:
             a.x.dense = dense.data_ptr()
             _cross_ck(lib.exb_cross_bwd(ctypes.byref(a), st), "cross_bwd")
 
+    # ---- AutoInt: the field self-attention (csrc/cuda/autoint_kernels.cu + the wgmma GEMM), buffers allocated once
+    def _att_init_buffers(self):
+        B, nf, La, dev = self.B, self.nf, self.att_layers, self.dev
+        f32, bf16 = torch.float32, torch.bfloat16
+        dh, Np, Kp = self.att_dh, self.att_Np, self.att_Kp
+        self.att_lib = _att_lib()
+        self.att_R = R = B * nf             # rows (sample, field)
+        self.att_X = [torch.zeros(R, Kp[l], dtype=bf16, device=dev) for l in range(La)]        # layer inputs (GEMM A)
+        self.att_QKVR = [torch.zeros(R, Np, dtype=f32, device=dev) for _ in range(La)]          # projections
+        self.att_P = [torch.zeros(B, self.att_h, nf, nf, dtype=f32, device=dev) for _ in range(La)]   # softmax
+        self.att_Xf = [torch.zeros(R, dh, dtype=f32, device=dev) for _ in range(La)]            # layer outputs
+        self.att_dQKVR = [torch.zeros(R, Np, dtype=bf16, device=dev) for _ in range(La)]
+        self.att_dX = [torch.zeros(R, Kp[l], dtype=f32, device=dev) for l in range(La)]         # input gradients
+        self.att_gpart = torch.zeros((B + 127) // 128, nf * dh, dtype=f32, device=dev)          # g_watt partial sums
+        p = lambda t: t.data_ptr() if t is not None else 0
+        watt, res = self.view("watt").data_ptr(), int(self.att_res)
+        self._att_fwd_args, self._att_bwd_args = [], []
+        for l in range(La):
+            last = l == La - 1
+            self._att_fwd_args.append(_AttFwdArgs(
+                p(self.att_QKVR[l]), Np, p(self.att_P[l]), p(self.att_Xf[l]), 0 if last else p(self.att_X[l + 1]),
+                0 if last else Kp[l + 1], watt if last else 0, p(self.base) if last else 0, B, nf, self.att_d,
+                self.att_h, res))
+            self._att_bwd_args.append(_AttBwdArgs(
+                p(self.att_QKVR[l]), Np, p(self.att_P[l]), p(self.att_Xf[l]), 0 if last else p(self.att_dX[l + 1]),
+                0 if last else Kp[l + 1], p(self.dlogit) if last else 0, watt if last else 0, p(self.att_dQKVR[l]),
+                p(self.att_gpart) if last else 0, B, nf, self.att_d, self.att_h, res, 0))
+        # split-K of the weight-gradient GEMMs (K = R rows): about two waves of output tiles
+        self.att_splits = [max(1, min(R // 1024, 264 // ((Kp[l] // 128 + 1) * (Np // 128 + 1)))) for l in range(La)]
+
+    def _att_forward(self, st):
+        """layer 0's operand from X32, then the projection and attention of every layer; the last adds
+        flatten(X_L) . w_att to base (after the forward GEMMs, before the head)"""
+        lib, R, Np, Kp = self.att_lib, self.att_R, self.att_Np, self.att_Kp
+        _att_ck(lib.exb_att_gather(self.X32.data_ptr(), self.XS, self.Dp, self.D, self.nf, self.att_X[0].data_ptr(),
+                                   Kp[0], self.B, st), "att_gather")
+        for l in range(self.att_layers):
+            G.gemm_nt(self.att_X[l], self.aWTb[l], R, Np, Kp[l], self.att_QKVR[l], mode=G.EPI_DX_FM, fm_cols=0, stream=st)
+            _att_ck(lib.exb_att_fwd(ctypes.byref(self._att_fwd_args[l]), st), "att_fwd")
+
+    def _att_backward(self, st):
+        """per layer from the last: [dQ | dK | dV | dR], the weight gradient, the input gradient; then the fold of
+        layer 0's input gradient into G32 (after the DNN's dX GEMM wrote those columns, before cachegrad and the push)
+        and of g_watt's partial sums into gtheta"""
+        lib, R, Np, Kp = self.att_lib, self.att_R, self.att_Np, self.att_Kp
+        for l in range(self.att_layers - 1, -1, -1):
+            _att_ck(lib.exb_att_bwd(ctypes.byref(self._att_bwd_args[l]), st), "att_bwd")
+            G.gemm_tn(self.att_X[l], self.att_dQKVR[l], Kp[l], Np, R, self.aview(l, grad=True),
+                      splits=self.att_splits[l], stream=st)
+            G.gemm_nt(self.att_dQKVR[l], self.aWb[l], R, Kp[l], Np, self.att_dX[l], mode=G.EPI_DX_FM, fm_cols=0,
+                      stream=st)
+        _att_ck(lib.exb_att_fold(self.G32.data_ptr(), self.XS, self.Dp, self.D, self.nf, self.att_dX[0].data_ptr(),
+                                 Kp[0], self.B, self.att_gpart.data_ptr(), self.nf * self.att_dh,
+                                 self.gview("watt").data_ptr(), st), "att_fold")
+
     def _st(self):
         return torch.cuda.current_stream(self.dev).cuda_stream
 
@@ -787,6 +961,9 @@ class FusedCTR:
         for l in range(self.cross_layers):
             _ck(self.lib.exb_refresh_bf16(self.view("X%d" % l).data_ptr(), self.xWb[l].data_ptr(), self.xWTb[l].data_ptr(),
                                           self.K0p, self.K0p, self._st()), "refresh_bf16")
+        for l in range(self.att_layers):
+            _ck(self.lib.exb_refresh_bf16(self.view("T%d" % l).data_ptr(), self.aWb[l].data_ptr(), self.aWTb[l].data_ptr(),
+                                          self.att_Kp[l], self.att_Np, self._st()), "refresh_bf16")
 
     def _forward(self, ids, dense, st, loss, opt_step):
         """prep, the forward GEMMs and the CIN / cross branches on the rows in X32: leaves H[-1] and base for a
@@ -815,6 +992,9 @@ class FusedCTR:
         if self.dcn:
             self._cross_forward(st, dense)
             self._mark("cross_fwd")
+        if self.autoint:
+            self._att_forward(st)
+            self._mark("att_fwd")
 
     # ---- forward-only pass (evaluation; all launches on the current stream)
     def predict_forward(self, ids, dense):
@@ -841,6 +1021,7 @@ class FusedCTR:
         n = 1 + prep + (1 if self.chain_fwd else L) + 1                # pull prep GEMMs head
         n += 2 + 2 * len(self.cin_layers) if self.cin else 0          # gather + pool, per layer outer + GEMM
         n += 2 * self.cross_layers if self.dcn else 0                 # per layer GEMM + cross forward
+        n += 1 + 2 * self.att_layers if self.autoint else 0           # gather, per layer GEMM + attention forward
         return n + (1 if metric else 0)
 
     # ---- one training step (all launches on the current stream)
@@ -895,6 +1076,9 @@ class FusedCTR:
         if self.dcn:
             self._cross_backward(st, dense)
             self._mark("cross_bwd")
+        if self.autoint:
+            self._att_backward(st)
+            self._mark("att_bwd")
         forked = update and self.overlap
         if forked:
             cur = torch.cuda.current_stream(self.dev)
@@ -991,6 +1175,8 @@ class FusedCTR:
         n += 3 + 6 * len(self.cin_layers) if self.cin else 0
         # DCN-v2: per layer GEMM + cross forward; backward top, per layer P GEMM + weight-gradient GEMM + cross backward
         n += 1 + 5 * self.cross_layers if self.dcn else 0
+        # AutoInt: gather + fold, per layer projection GEMM + attention forward, attention backward + two GEMMs
+        n += 2 + 5 * self.att_layers if self.autoint else 0
         return n + (1 if self._ar is not None and not self._rider else 0)
 
     # ---- dense state, checkpoints and export (all through ``self.layout``)
@@ -1000,7 +1186,10 @@ class FusedCTR:
                 "num_dense": self.nd, "hidden": list(self.hidden), "cin_layers": list(self.cin_layers),
                 "cin_split_half": self.cin_split_half if self.cin else None, "cross_layers": self.cross_layers,
                 "pack_linear": self.pack_linear, "batch": self.B, "world": self.ctx.world,
-                "dense_optimizer": self.dense_opt["category"]}
+                "dense_optimizer": self.dense_opt["category"], "att_layers": self.att_layers or None,
+                "att_embedding_size": self.att_d if self.autoint else None,
+                "att_head_num": self.att_h if self.autoint else None,
+                "att_res": self.att_res if self.autoint else None}
 
     def config_mismatches(self, config):
         """one line per configuration entry in which ``config`` differs from this model's"""
@@ -1106,7 +1295,9 @@ class FusedCTR:
             raise ValueError("can not convert sparse variable to nn.Embedding.")
         mod = StandaloneCTR(self.vocab, num_dense=self.nd, embedding_dim=self.D, model=self.model, hidden=self.hidden,
                             cached=self.cached, cin_layers=self.cin_layers or (128, 128),
-                            cin_split_half=self.cin_split_half, cross_layers=self.cross_layers or 3)
+                            cin_split_half=self.cin_split_half, cross_layers=self.cross_layers or 3,
+                            **(dict(att_layers=self.att_layers, att_embedding_size=self.att_d, att_head_num=self.att_h,
+                                    att_res=self.att_res) if self.autoint else {}))
         sd = self.dense_state_dict(include_optimizer=False)
         sd["bias"] = sd["bias"] + sd.pop("dnn_out.bias")
         missing, unexpected = mod.load_state_dict(sd, strict=False)
@@ -1191,6 +1382,8 @@ class FusedCTR:
             z = z + self._reference_cin(emb.view(B, nf, Dp)[:, :, :self.D], theta)
         if self.dcn:
             z = z + self._reference_cross(torch.cat([emb.view(B, nf, Dp)[:, :, :self.D].reshape(B, -1), dense], 1), theta)
+        if self.autoint:
+            z = z + self._reference_att(emb.view(B, nf, Dp)[:, :, :self.D], theta)
         loss =torch.nn.functional.binary_cross_entropy_with_logits(z, labels)
         loss.backward()
         grads = {"theta": theta.grad, "emb": emb_leaf.grad, "lin": lin_leaf.grad}
@@ -1250,6 +1443,26 @@ class FusedCTR:
         xL = torch.func.functional_call(self._ref_cross, params, (x,))
         o, n = self.segs["wcross"]
         return xL @ theta[o:o + n][cols]
+
+
+    def _reference_att(self, x, theta):
+        """flatten(AutoInt(x)) . w_att for ``reference``: the eager zoo's ``InteractingLayer.attend`` (plain torch, fp32)
+        on the projections of the stacked weights in ``theta``, rounded to bf16 where the kernels round -- X_l and T_l
+        on the way into the projection GEMM with an fp32 gradient passed straight through, and the gradient of the
+        projections (the kernels' bf16 [dQ | dK | dV | dR]). The projections themselves stay fp32. x: [B, nf, D]."""
+        from .ctr import InteractingLayer
+        bf16 = torch.bfloat16
+        st = lambda t: t + (t.to(bf16).float() - t).detach()        # bf16 value, fp32 gradient
+        dh = self.att_dh
+        for l in range(self.att_layers):
+            o, sz = self.segs["T%d" % l]
+            T = st(theta[o:o + sz].view(self.att_Kp[l], self.att_Np))[:x.shape[-1]]
+            proj = st(x) @ T
+            proj.register_hook(lambda g: g.to(bf16).float())
+            q, k, v = proj[..., :dh], proj[..., dh:2 * dh], proj[..., 2 * dh:3 * dh]
+            x = InteractingLayer.attend(q, k, v, proj[..., 3 * dh:4 * dh] if self.att_res else None, self.att_h)
+        o, n = self.segs["watt"]
+        return x.reshape(x.shape[0], -1) @ theta[o:o + n]
 
 
 class FusedTrainer:
